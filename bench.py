@@ -1,36 +1,43 @@
 #!/usr/bin/env python
-"""bench.py -- ELF-strip throughput of the B200 path vs the reference's host `strip` pipeline.
+"""bench.py -- ELF-strip throughput of the H100 path vs the reference's host `strip` pipeline.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W]              # this repo (CUDA kernels)
-  python bench.py --impl reference [--gpus N] [--steps K] ...      # the reference's CPU pipeline
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   # this repo (CUDA kernels)
+  python bench.py --impl reference [--gpus N] [--steps K] ...                # the reference's CPU pipeline
 
 Metric (BASELINE.json): ELF-strip GB/s of build-tree `.so` INPUT bytes.
 
-Workload (default, `--scaling strong`) = BASELINE config 4 as stated: the synthetic corpus of 10 000 `.so`
-files, sizes log-uniform 1 KB..128 MB (seed 0xB200, dropped fraction U(0.05,0.8); 115 GB in, 67 GB out),
-dealt size-sorted round-robin over the N ranks -- the SAME 10 000 files at every N (at N=8 this is also
-config 5, "100 GB over 8 B200").  One "step" = one pass of the hot path over the rank's whole shard.  A
-shard whose input + output does not fit in HBM side by side (N=1: 115 + 67 GB) keeps the input resident
-and streams the output through a two-slot ring (lb2_strip_device_chunked), one batch per ~14 GB chunk.
-`--scaling weak` is round 1's workload (1250 files per GPU).  No payload crosses GPUs; the one collective
-is a single NCCL allgather of the per-rank byte counts after the last step, inside the timed region.
+Workload (default, `--scaling strong`): the synthetic corpus of BASELINE config 4 (sizes log-uniform
+1 KB..128 MB, seed 0xB200, dropped fraction U(0.05,0.8)) sized for one 80 GB H100: 2 500 `.so` files,
+~26 GB in and ~15 GB out, so that input and output arenas sit side by side in HBM at N=1.  Files are dealt
+size-sorted round-robin over the N ranks -- the SAME files at every N.  One "step" = one pass of the hot
+path over the rank's whole shard.  A shard whose input + output does not fit in HBM side by side (a larger
+--total-files) keeps the input resident and streams the output through a two-slot ring
+(lb2_strip_device_chunked), one batch per --chunk-gb chunk.  `--scaling weak` gives every GPU
+--files-per-gpu files.  No payload crosses GPUs; the one collective is a single NCCL allgather of the
+per-rank byte counts after the last step, inside the timed region.
 
   value      device-resident: inputs already in HBM; timed = upload of offsets + plan kernel + offset scan +
              compaction kernel + fetch of sizes/status per batch, + the allgather.  CUDA events, max over ranks.
   e2e        the same hot path through the C ABI with HOST buffers (lb2_strip_host on pinned arenas placed on
              the GPU's NUMA node): headers and kept extents cross PCIe up, stripped files come down, inside the
-             timed region.  Host memory bounds it to the first <= 15 GB of each rank's shard.
+             timed region.  Host memory bounds it to the first <= 8 GiB of each rank's shard.
   tree       (N=1) lb2_strip_tree -- the call that replaces project_build.py:260 -- on a /dev/shm tree holding
              the same files the reference arm strips: file reads and in-place writes included.
   roofline   compaction kernel: algorithmic bytes (copied extents read + output written) over its CUDA-event
-             duration against MEASURED_PEAKS.json hbm_gbs; every rank's figure is in `per_rank`.
+             duration against the HBM copy rate measured at start-up on the same GPU (device-to-device copy of
+             1 GiB, best of 12; MEASURED_PEAKS.json hbm_gbs instead when present); every rank's figure is in
+             `per_rank`.
   cpu_baseline / --impl reference: the reference's own line `find DIR/ -name "*.so" | xargs strip`
-             (/root/reference/lambdipy/project_build.py:260) on /dev/shm over the first <= 15 GB of the
-             corpus (1/8: ~1250 files): serial as the reference runs it, and `xargs -P nproc -n 1`.
+             (lambdipy/project_build.py:260) on /dev/shm over the first <= 8 GiB of the corpus: serial as the
+             reference runs it, and `xargs -P nproc -n 1`.
   parity     after the timed region every rank strips 8 size-stratified files of ITS shard with the real
              `strip --strip-unneeded` and compares them byte for byte with what the GPU produced.
   real_trees (N=1) BASELINE configs 2 and 3 (stand-ins from this image's site-packages): kernels, tree call,
              reference line, fallback count.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned to its caller
+(per-file status, output sizes and offsets, the batch counters, and a fixed seeded sample of the
+stripped bytes) as float64 / float32 .npy files, so that two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -48,11 +55,13 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 METRIC = "ELF-strip GB/s (build-tree .so bytes)"
-TOTAL_FILES = 10000
+TOTAL_FILES = 2500            # ~26 GB in + ~15 GB out: both arenas fit one 80 GB H100
 FILES_PER_GPU = 1250
 SEED = 0xB200
-SAMPLE_SPAN = 15 << 30        # host-side legs (e2e, tree, CPU baseline) work on the first <= 15 GiB of a shard
+SAMPLE_SPAN = 8 << 30         # host-side legs (e2e, tree, CPU baseline) work on the first <= 8 GiB of a shard
 LAUNCHES_PER_BATCH = 3        # plan, scan (+ tile expansion of the very big extents), compaction
+DUMP_WINDOWS, DUMP_WINDOW_BYTES = 256, 32 << 10  # --dump-outputs: seeded byte windows of the stripped output
+DUMP_EDGE_FILES, DUMP_EDGE_BYTES = 64, 4096      # ... and the first / last bytes (regenerated headers) of seeded files
 
 
 def peaks():
@@ -60,7 +69,23 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured)"
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md; MEASURED_PEAKS.json absent)"
+    import torch
+    n = 1 << 30
+    a = torch.empty(n, dtype=torch.uint8, device="cuda")
+    b = torch.empty_like(a)
+    a.fill_(1)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    best = None
+    for _ in range(12):
+        e0.record()
+        b.copy_(a)
+        e1.record()
+        e1.synchronize()
+        ms = e0.elapsed_time(e1)
+        best = ms if best is None else min(best, ms)
+    del a, b
+    torch.cuda.empty_cache()
+    return 2 * n / 1e9 / (best / 1e3), "measured in this run: device-to-device copy of 1 GiB, read + write bytes, best of 12"
 
 
 # ---------------------------------------------------------------- clocks during the timed region
@@ -284,8 +309,8 @@ def sample_count(corpus):
 
 def workload_config(a, world):
     if a.scaling == "strong":
-        w = ("synthetic ELF corpus, BASELINE config 4 at full size (= config 5 at 8 GPUs): %d files, sizes log-uniform 1 KB-128 MB, "
-             "seed 0x%X, dropped fraction U(0.05,0.8), ~115 GB in / ~67 GB out; the same files at every N, dealt size-sorted "
+        w = ("synthetic ELF corpus (BASELINE config 4 generator, sized for one 80 GB H100): %d files, sizes log-uniform 1 KB-128 MB, "
+             "seed 0x%X, dropped fraction U(0.05,0.8); the same files at every N, dealt size-sorted "
              "round-robin over %d rank(s)" % (a.total_files, SEED, world))
     else:
         w = ("synthetic ELF corpus (BASELINE config 4/5 generator): %d files per GPU (%d total), sizes log-uniform 1 KB-128 MB, "
@@ -293,7 +318,7 @@ def workload_config(a, world):
              (a.files_per_gpu, a.files_per_gpu * world, SEED))
     return {"workload": w, "total_files": a.total_files if a.scaling == "strong" else a.files_per_gpu * world,
             "parallelism": "file-sharded x%d, no payload exchange, one allgather of byte counts" % world,
-            "l2": "inputs (>10 GB per GPU) far larger than the 126 MB L2; no flush needed"}
+            "l2": "inputs (GBs per GPU) far larger than the 50 MB L2; no flush needed"}
 
 
 def _materialize(args):
@@ -318,25 +343,17 @@ def run_reference(a, rank, world):
         jobs = [(corpus, i, os.path.join(master, "f%05d.so" % i)) for i in range(ns)]
         with Pool(min(48, os.cpu_count() or 1)) as pool:
             pool.map(_materialize, jobs, chunksize=2)
-        # bound the run: K timed + W warm-up parallel runs must end within a few minutes; the serial line once
-        t_probe0 = time.perf_counter()
-        res = cpu_lines_on_master(base, master, n_bytes, 1, 0, 1)
-        per_run = (time.perf_counter() - t_probe0) / 2
-        budget = 240.0
-        steps = max(1, min(a.steps, int(budget / max(per_run, 1e-3)) - 1))
-        warm = max(0, min(a.warmup, steps // 4))
-        more = cpu_lines_on_master(base, master, n_bytes, steps, warm, 0) if steps > 1 else None
-        if more:
-            res["parallel_s"] = more["parallel_s"]; res["parallel_gbs"] = more["parallel_gbs"]
+        # --steps timed parallel runs after --warmup untimed ones; the serial line once
+        res = cpu_lines_on_master(base, master, n_bytes, a.steps, a.warmup, 1)
     finally:
         shutil.rmtree(base, ignore_errors=True)
     value = res["parallel_gbs"]
     sample = ("the first %d files (%.3f GB, 1 KB-128 MB each) of the corpus on /dev/shm, every timed run on a fresh copy; `%s` "
-              "(GNU strip: %s) with all %d host cores; %d timed runs%s; serial as the reference runs it (1 process): %.3f GB/s"
+              "(GNU strip: %s) with all %d host cores; %d timed runs; serial as the reference runs it (1 process): %.3f GB/s"
               % (ns, n_bytes / 1e9, PAR_LINE.format(d="DIR", p=res["nproc"]), strip_version(), res["nproc"], len(res["parallel_s"]),
-                 "" if len(res["parallel_s"]) == a.steps else " (of --steps %d: bounded to a few minutes)" % a.steps, res["serial_gbs"] or 0))
+                 res["serial_gbs"] or 0))
     line = {
-        "impl": "reference", "metric": METRIC, "value": value, "unit": "GB/s", "n_gpus": a.gpus, "steps": a.steps,
+        "impl": "reference", "metric": METRIC, "value": value, "unit": "GB/s", "n_gpus": a.gpus, "steps": len(res["parallel_s"]),
         "warmup": a.warmup, "ms_per_step": 1e3 * sum(res["parallel_s"]) / len(res["parallel_s"]),
         "higher_is_better": True, "scaling": a.scaling, "vs_baseline": None, "dtype": "u8", "data": "synthetic",
         "config": workload_config(a, world),
@@ -420,7 +437,77 @@ def real_trees_block(ctx, peak):
     return out
 
 
-# ---------------------------------------------------------------- B200 arm
+# ---------------------------------------------------------------- --dump-outputs
+def dump_windows(sizes, n_windows):
+    """(file, start, length) of the bytes sampled from the stripped output: windows at seeded positions of the
+    concatenated output, then the first and last bytes (regenerated Ehdr/Phdr and Shdr tables) of seeded files."""
+    import numpy as np
+    sizes = np.asarray(sizes, dtype=np.int64)
+    ends = np.cumsum(sizes)
+    total = int(ends[-1]) if len(sizes) else 0
+    rng = np.random.default_rng(SEED)
+    out = []
+    if total == 0:
+        return out
+    for p in np.sort(rng.integers(0, total, size=n_windows)):
+        i = int(np.searchsorted(ends, p, side="right"))
+        start = int(p - (ends[i] - sizes[i]))
+        out.append((i, start, min(DUMP_WINDOW_BYTES, int(sizes[i]) - start)))
+    nz = np.flatnonzero(sizes)
+    for i in np.sort(rng.choice(nz, size=min(DUMP_EDGE_FILES, len(nz)), replace=False)):
+        m = min(DUMP_EDGE_BYTES, int(sizes[i]))
+        out.append((int(i), 0, m))
+        out.append((int(i), int(sizes[i]) - m, m))
+    return out
+
+
+def dump_outputs(d, ctx, batch, st, chunked, stream, rank, world):
+    """What the last timed step returned to its caller, as DIR/<name>.npy.  A chunked shard's ring keeps only its
+    last two chunks, so there the output bytes and per-chunk offsets come from one more (untimed) pass over the
+    same inputs."""
+    import numpy as np
+    n = batch.n
+    windows = dump_windows(batch.out_sizes[:n], max(1, DUMP_WINDOWS // world))
+    offs = batch.out_off[:n].astype(np.float64)
+    got = {}
+
+    def read(k, base):
+        i, start, m = windows[k]
+        buf = C.create_string_buffer(max(m, 1))
+        ctx.d2h(buf, base + start, m)
+        got[k] = buf.raw[:m]
+
+    if chunked:
+        by_file = {}
+        for k, (i, _, _) in enumerate(windows):
+            by_file.setdefault(i, []).append(k)
+
+        def grab(chunk, f0, cnt, d_slot, ooff, osz, stat):
+            for j in range(cnt):
+                offs[f0 + j] = float(ooff[j])  # relative to the chunk's output slot
+                for k in by_file.get(f0 + j, ()):
+                    read(k, d_slot + int(ooff[j]))
+        batch.strip_chunked(stream=stream, on_chunk=grab)
+    else:
+        for k, (i, _, _) in enumerate(windows):
+            read(k, batch.d_out + int(batch.out_off[i]))
+    sample = b"".join(got[k] for k in range(len(windows)))
+    prefix = "" if world == 1 else "rank%d_" % rank
+    arrays = {
+        "status": batch.status[:n].astype(np.float64),
+        "out_sizes": batch.out_sizes[:n].astype(np.float64),
+        "out_off": offs,
+        "counters": np.array([st[k] for k in ("n_ok", "n_unsupported", "in_bytes", "out_bytes", "copy_bytes", "header_bytes", "n_tiles")],
+                             dtype=np.float64),
+        "sample_windows": np.array(windows, dtype=np.float64).reshape(-1, 3),
+        "sample_bytes": np.frombuffer(sample, dtype=np.uint8).astype(np.float32),
+    }
+    os.makedirs(d, exist_ok=True)
+    for name, arr in arrays.items():
+        np.save(os.path.join(d, prefix + name + ".npy"), arr)
+
+
+# ---------------------------------------------------------------- CUDA arm
 def run_b200(a, rank, local_rank, world):
     # NCCL's own INIT lines (communicator, nranks, transport) stay visible on its default sink (stdout; pointing
     # NCCL_DEBUG_FILE at /dev/stderr lost them on the GPU box).  The JSON line is the LAST line rank 0 prints.
@@ -443,10 +530,9 @@ def run_b200(a, rank, local_rank, world):
     n = len(corpus)
     in_span = int(corpus.off[-1])
     free_b, total_b = torch.cuda.mem_get_info()
-    # A shard whose input + output exceed HBM (N=1: 115 + 67 GB) keeps the input resident and streams the output through
-    # the two-slot ring of lb2_strip_device_chunked; otherwise one batch per step (splitting a shard that fits into two
-    # pipelined batches was measured: 2.84 vs 2.79 ms per step at N=8 -- the second plan/scan costs more than the hidden
-    # host round trip).
+    # A shard whose input + output exceed HBM keeps the input resident and streams the output through the two-slot ring
+    # of lb2_strip_device_chunked; otherwise one batch per step (a second plan/scan per step costs more than the host
+    # round trip that splitting a shard into two pipelined batches would hide).
     big = (2 * in_span + n * 4096 + (1 << 30)) > 0.85 * free_b
     chunked = big
     chunk_bytes = int(a.chunk_gb * (1 << 30)) if big else None
@@ -511,6 +597,8 @@ def run_b200(a, rank, local_rank, world):
         assert int(g[:, 2].sum()) == total_files and int(g[:, 3].sum()) == 0, g
     cms, pms = sum(compact_ms) / len(compact_ms), sum(plan_ms) / len(plan_ms)
     alg = st["copy_bytes"] + st["out_bytes"]
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, ctx, batch, st, chunked, sptr, rank, world)
     if a.profile_mode:
         if rank == 0:
             print(json.dumps({"profile_mode": True, "ms_per_step": dev_ms / a.steps, "compact_ms": compact_ms, "plan_ms": plan_ms,
@@ -543,7 +631,7 @@ def run_b200(a, rank, local_rank, world):
         mismatches += (want is None) or (want != got.get(i))
     shutil.rmtree(pdir, ignore_errors=True)
 
-    # ---- end to end through host buffers (the first <= 15 GiB of the shard)
+    # ---- end to end through host buffers (the first <= SAMPLE_SPAN bytes of the shard)
     ns = sample_count(corpus) if in_span > SAMPLE_SPAN else n
     s_span = int(corpus.off[ns])
     h_in = ctx.pinned_alloc(s_span + 256)
@@ -748,12 +836,15 @@ def main():
     ap.add_argument("--scaling", default="strong", choices=["strong", "weak"])
     ap.add_argument("--total-files", type=int, default=TOTAL_FILES, help="strong scaling: files in the whole corpus")
     ap.add_argument("--files-per-gpu", type=int, default=FILES_PER_GPU, help="weak scaling: files per GPU")
-    ap.add_argument("--chunk-gb", type=float, default=14.0, help="output-ring chunk when input + output exceed HBM")
+    ap.add_argument("--chunk-gb", type=float, default=6.0, help="output-ring chunk when input + output exceed HBM")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last step returned as DIR/<name>.npy")
     ap.add_argument("--e2e-steps", type=int, default=5)
     ap.add_argument("--no-host-legs", action="store_true", help="skip cpu_baseline / tree / real_trees (N=1)")
     ap.add_argument("--no-real-trees", action="store_true")
     ap.add_argument("--profile-mode", action="store_true", help="device-resident steps only (for runs under ncu; not a bench value)")
     a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -1,5 +1,5 @@
 /*
- * lambdipy_b200.h -- C ABI of the B200 (sm_100a) ELF strip library, liblambdipy_b200.so.
+ * lambdipy_b200.h -- C ABI of the H100 (sm_90a) ELF strip library, liblambdipy_b200.so.
  *
  * What it replaces.  The reference (customink/lambdipy) has no FFI for this step: it strips the
  * build tree by running one shell line inside a generated script,
@@ -144,8 +144,7 @@ int lb2_batch_results(lb2_ctx *ctx, uint64_t *h_out_off /* n+1 */, uint64_t *h_o
  * slot is reused two chunks later -- the consumer owns the slot only for the duration of the callback.
  * Offsets passed to the callback are relative to the slot.  h_out_sizes / h_status (n_files each, may be
  * NULL) receive the per-file results; *total sums the chunks (plan_ms / compact_ms: summed kernel times).
- * This is what one `strip` process does to an argument list longer than memory: SURVEY.md D7, the
- * 10 000-file corpus of BASELINE config 4 on one GPU (/root/reference/lambdipy/project_build.py:260). */
+ * This is what one `strip` process does to an argument list longer than memory (SURVEY.md D7). */
 typedef int (*lb2_chunk_fn)(void *user, uint32_t chunk, uint32_t first_file, uint32_t n_files, const void *d_out_slot,
                             const uint64_t *out_off, const uint64_t *out_sizes, const int32_t *status,
                             const lb2_stats *chunk_stats);
@@ -160,7 +159,7 @@ int lb2_strip_device_chunked(lb2_ctx *ctx, const void *d_in, const uint64_t *h_i
  * kernels run on them directly over PCIe (zero-copy: only headers and kept extents are pulled, stripped
  * files are pushed straight back; LB2_HOST_ZEROCOPY=0 disables).  LB2_HOST_DMA=1 selects the copy-engine
  * variant instead: plan over the mapping, DMA of the kept ranges into a device slot, compaction in HBM, DMA
- * of the output (same bytes on the bus, measured within 3 % of zero-copy).  Otherwise, or when both are
+ * of the output (same bytes on the bus).  Otherwise, or when both are
  * disabled: explicit H2D of whole files -> kernels -> D2H, pipelined in <= LB2_CHUNK_MB (256) MB chunks of
  * whole files on three streams.  stats->h2d_bytes / d2h_bytes say what crossed the bus. */
 int lb2_strip_host(lb2_ctx *ctx, const void *h_in, const uint64_t *h_in_off, const uint64_t *h_in_sizes,

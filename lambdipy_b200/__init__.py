@@ -1,4 +1,4 @@
-"""lambdipy_b200 -- the shared-object strip pass of customink/lambdipy on B200 (sm_100a).
+"""lambdipy_b200 -- the shared-object strip pass of customink/lambdipy on H100 (sm_90a).
 
 Public surface:
     strip_tree(build_directory)                 replaces `find ... -name "*.so" | xargs strip`

@@ -2,7 +2,7 @@
 
 The library is CUDA-only: there is no CPU implementation behind it, and nothing here falls back
 to one.  `load()` raises if the shared object is missing (build it with
-`python -m lambdipy_b200.build`); `Context()` raises `NoDeviceError` without a B200.
+`python -m lambdipy_b200.build`); `Context()` raises `NoDeviceError` without an H100.
 """
 import ctypes as C
 import os

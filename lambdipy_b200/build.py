@@ -1,4 +1,4 @@
-"""Build liblambdipy_b200.so (sm_100a) in-tree with nvcc.  `python -m lambdipy_b200.build`."""
+"""Build liblambdipy_b200.so (sm_90a, H100) in-tree with nvcc.  `python -m lambdipy_b200.build`."""
 import os
 import subprocess
 import sys
@@ -9,7 +9,7 @@ OUT = os.path.join(HERE, "liblambdipy_b200.so")
 SOURCES = ["plan.cu", "compact.cu", "compact_tma.cu", "corpus.cu", "api.cu"]
 HEADERS = ["lb2_common.cuh", "copy_device.cuh", os.path.join("..", "..", "include", "lambdipy_b200.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "--shared", "-cudart", "shared",
 ]
 

@@ -70,7 +70,7 @@ struct lb2_ctx {
   int async_head = 0, async_count = 0;  // lb2_strip_device_async: up to two batches in flight (ws, ws2), collected in order
   std::string err;
   int compact_ctas_per_sm = 4;
-  int use_tma = 1;             // bulk-copy engine kernel (0.97 of copy peak) ; LB2_COMPACT_TMA=0 selects the LSU kernel (0.90)
+  int use_tma = 1;             // bulk-copy engine kernel; LB2_COMPACT_TMA=0 selects the LSU kernel
   // host pipeline slots
   struct Slot {
     Workspace ws;
@@ -94,8 +94,8 @@ static void tree_engine_free(TreeEngine *e);
   } while (0)
 
 // Pinned host arenas are placed on the NUMA node the GPU hangs off: the compaction kernel of the zero-copy
-// host path reads and writes them over PCIe at ~50 GB/s per direction, and a remote-socket arena puts that
-// traffic on the inter-socket link (round 1: 40 GB/s per direction at 1 GPU, half of that per GPU at 8).
+// host path reads and writes them over PCIe, and a remote-socket arena puts that traffic on the
+// inter-socket link as well.
 // The policy is set only around the allocation (MPOL_PREFERRED: falls back to other nodes when full).
 static int gpu_numa_node(int device) {
   char bus[64] = {0};
@@ -333,7 +333,7 @@ static int collect_batch(lb2_ctx *ctx, Workspace &w, uint64_t *h_out_off, uint64
 // ============================================================================ C ABI
 extern "C" {
 
-const char *lb2_version(void) { return "lambdipy_b200 0.1 (sm_100a; GNU strip 2.42 semantics)"; }
+const char *lb2_version(void) { return "lambdipy_b200 0.1 (sm_90a; GNU strip 2.42 semantics)"; }
 
 int lb2_ctx_create(int device, lb2_ctx **out) {
   if (!out) return LB2_E_ARG;
@@ -356,8 +356,8 @@ int lb2_ctx_create(int device, lb2_ctx **out) {
   cudaGetDeviceProperties(&prop, device);
   ctx->sm_count = prop.multiProcessorCount;
   ctx->numa_node = gpu_numa_node(device);
-  if (prop.major < 10) {
-    g_create_error = "this library is built for sm_100a (B200) only; device is sm_" + std::to_string(prop.major) + std::to_string(prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {  // sm_90a code loads on compute capability 9.0 only
+    g_create_error = "this library is built for sm_90a (H100) only; device is sm_" + std::to_string(prop.major) + std::to_string(prop.minor);
     cudaStreamDestroy(ctx->stream);
     delete ctx;
     return LB2_E_NODEVICE;
@@ -443,8 +443,8 @@ int lb2_plan_device(lb2_ctx *ctx, const void *d_in, const uint64_t *h_in_off, co
 }
 
 // ---------------------------------------------------------------------------- shards larger than HBM
-// A shard whose input plus output does not fit next to each other in HBM (BASELINE config 4 on one GPU:
-// 115 GB in + 67 GB out; SURVEY D7) keeps its INPUT resident and streams the OUTPUT through a ring of two
+// A shard whose input plus output does not fit next to each other in HBM keeps its INPUT resident and
+// streams the OUTPUT through a ring of two
 // slots: chunk k (consecutive files, <= max_chunk_bytes of arena span) is stripped into slot k % 2 while
 // the consumer still holds chunk k-1.  Chunk k+1 is queued on the stream before chunk k is collected, so
 // the GPU never waits for the host between chunks.
@@ -545,8 +545,7 @@ int lb2_strip_host(lb2_ctx *ctx, const void *h_in_v, const uint64_t *h_in_off, c
     cudaGetLastError();  // clear "invalid value" from probing pageable memory
     if (ok && env_u64("LB2_HOST_DMA", 0)) {
       // opt-in (LB2_HOST_DMA=1): plan over the mapping, copy-engine transfers of the kept ranges, compaction in HBM.
-      // Measured equal to the zero-copy path below within 3 % (67.9 vs 69.5 GB/s at 1 GPU, 312.6 vs 303.9 at 8):
-      // the copy engines' edge over SM loads/stores is eaten by the per-chunk plan -> host -> DMA hand-over.
+      // The copy engines' edge over SM loads/stores is largely eaten by the per-chunk plan -> host -> DMA hand-over.
       return strip_host_dma(ctx, h_in, static_cast<const uint8_t *>(d_in_alias), h_in_off, h_in_sizes, n_files, h_out, out_capacity,
                             h_out_off, h_out_sizes, h_status, flags, stats);
     }
@@ -675,9 +674,9 @@ int lb2_strip_host(lb2_ctx *ctx, const void *h_in_v, const uint64_t *h_in_off, c
 
 
 // ---- host buffers, pinned and mapped: plan over the mapping, upload only what is kept, compact in HBM ----------
-// Measured on this box (profiles/r02_pcie_probe.txt): the copy engines move 49.6 GB/s per direction with both
-// directions busy, SM loads/stores on mapped host memory 40.6 (what the zero-copy path gets).  So, per chunk of
-// whole files (<= LB2_CHUNK_MB of arena span, three slots rotating):
+// The copy engines move more bytes per second over PCIe than SM loads/stores on mapped host memory (what the
+// zero-copy path gets; tools/pcie_probe.cu measures both).  So, per chunk of whole files (<= LB2_CHUNK_MB of
+// arena span, three slots rotating):
 //   1. plan + scan run on the host-mapped input: only headers, names and notes cross the bus; the kernel also
 //      lists the input ranges its copy extents read (small files whole, neighbours merged);
 //   2. those ranges are uploaded by the copy engine into a device slot laid out like the host arena -- dropped

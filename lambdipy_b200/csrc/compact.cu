@@ -4,11 +4,11 @@
 // tables, .shstrtab, merged notes) or zero-filled (the file holes BFD leaves between sections).
 //
 // Pure byte movement -- no tensor cores.  Roofline: HBM read+write (SURVEY.md 8d).
-//   * lb2_compact_tma_kernel  (compact_tma.cu, default) bulk-copy engine path: 0.977 of the measured copy peak.
+//   * lb2_compact_tma_kernel  (compact_tma.cu, default) bulk-copy engine path.
 //   * lb2_compact_kernel      (this file; LB2_COMPACT_TMA=0, and lb2_corpus_scatter) warp-per-tile, 16-byte
 //                             vectorised LDG/STG, 8 loads in flight per lane, byte-granular heads/tails,
 //                             funnel-shifted path for tiles whose source and destination are not congruent
-//                             mod 16: 0.905 of the copy peak.
+//                             mod 16.
 //
 // Replaces the data movement GNU strip does with read()/write() per file
 // (/root/reference/lambdipy/project_build.py:260).

@@ -4,7 +4,7 @@
 // lane per CTA drive the engine, the remaining warps take what the engine cannot: heads/tails of
 // < 16 bytes, tiles whose source and destination are not congruent mod 16, zero fills.
 //
-// One persistent CTA per SM (grid = SM count); tiles are claimed dynamically.  SASS: UBLKCP (see profiles/).
+// One persistent CTA per SM (grid = SM count); tiles are claimed dynamically.  SASS: UBLKCP.
 #include "lb2_common.cuh"
 #include "copy_device.cuh"
 
@@ -68,7 +68,7 @@ __device__ __forceinline__ BulkSplit bulk_split(const TileView &v) {
 // `claim_help` feeds the helper warps, 32 tiles per claim.  Every tile is therefore visited twice, once
 // per role, by whichever CTA gets there first -- a CTA that starts late or shares its SM with a foreign
 // kernel (an NCCL collective on another stream) simply claims less, instead of stretching the kernel by
-// its whole static share (round-1 finding: 0.98 -> 0.64 of the copy peak at 8 GPUs with a static stride).
+// its whole static share.
 //
 // Inside a CTA the producer lane is the only one that sees tile descriptors of engine tiles: it posts
 // {destination, bytes} of each stage next to the stage, the storer lane picks them up after the full

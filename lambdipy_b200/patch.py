@@ -1,4 +1,4 @@
-"""Drop-in installation: make an installed `lambdipy` use the B200 strip path, CLI unchanged.
+"""Drop-in installation: make an installed `lambdipy` use the CUDA strip path, CLI unchanged.
 
     import lambdipy_b200.patch; lambdipy_b200.patch.apply()      # or: python -m lambdipy_b200.patch build ...
 

@@ -7,12 +7,12 @@ Reference: lambdipy.project_build.install_non_resolved_requirements
 (:260) -- runs it on the host (:268) or in a lambci container (:274) and deletes it (:277).
 
 This mirror keeps the signature, the printed messages, the script (minus its last line) and the
-exit-code convention, and performs the strip with the B200 library on the build tree once the
+exit-code convention, and performs the strip with the CUDA library on the build tree once the
 script has finished.  Nothing else of the reference is re-implemented here: requirement
 resolution, Docker builds, release download stay in the reference package (see patch.py).
 
 Backend switch (additive; the reference's TODO at cli.py:34-39 asks for one):
-    LAMBDIPY_STRIP_BACKEND=b200   default: CUDA path; raises if no B200 / library is present
+    LAMBDIPY_STRIP_BACKEND=b200   default: CUDA path; raises if no H100 / library is present
     LAMBDIPY_STRIP_BACKEND=gnu    the reference's own shell line, untouched
     LAMBDIPY_STRIP_BACKEND=off    do not strip
 """

@@ -1,4 +1,4 @@
-"""Host-side entry points of the B200 strip path.
+"""Host-side entry points of the CUDA strip path.
 
 `strip_tree(build_directory)` is the call that replaces the reference's shell line
 `find {install_dir}/ -name "*.so" | xargs strip` (/root/reference/lambdipy/project_build.py:260);

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Runs the REFERENCE's own install_non_resolved_requirements (imported from /root/reference with
-its missing third-party imports stubbed) on a scratch tree and records (a) the script it generates
-and (b) the file list / sizes after its strip, as tests/golden/ref_script.json.  Build container
-only; the GPU box checks the mirror in lambdipy_b200/project_build.py against this record."""
+"""Runs the REFERENCE's own install_non_resolved_requirements (imported from a checkout of
+customink/lambdipy given on the command line, its missing third-party imports stubbed) on a scratch
+tree and records (a) the script it generates and (b) the file list / sizes after its strip, as
+tests/golden/ref_script.json.  The tests check the mirror in lambdipy_b200/project_build.py against
+this record, so they do not need the reference."""
 import contextlib
 import io
 import json
@@ -24,7 +25,9 @@ for name in ("docker", "requirementslib", "github", "github.GithubException", "g
     m.UnknownObjectException = Exception
     m.GitRelease = object
     sys.modules[name] = m
-sys.path.insert(0, "/root/reference")
+if len(sys.argv) != 2:
+    sys.exit("usage: make_ref_script_golden.py <checkout of customink/lambdipy>")
+sys.path.insert(0, sys.argv[1])
 from lambdipy import project_build as ref  # noqa: E402
 
 

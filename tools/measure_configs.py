@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Measures BASELINE.json configs 1-3 (real build trees of this image) on the GPU box and prints one
-JSON document: for each tree the reference's own line on host cores (serial, and -P nproc), the
-B200 path device-resident (plan / compaction kernel times, roofline fraction), through host buffers
+"""Measures BASELINE.json configs 1-3 (real build trees of the installed packages) on a GPU machine and
+prints one JSON document: for each tree the reference's own line on host cores (serial, and -P nproc), the
+CUDA path device-resident (plan / compaction kernel times, roofline fraction), through host buffers
 (lb2_strip_host) and through the in-place tree API (lb2_strip_tree) -- plus a byte-for-byte check of
 the GPU-stripped tree against the reference-stripped tree.
 
@@ -22,6 +22,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np  # noqa: E402
 
 import elf_fixtures as F  # noqa: E402
+from bench import peaks  # noqa: E402  (the HBM copy rate of this GPU, measured the way bench.py measures it)
 from lambdipy_b200 import _native as N  # noqa: E402
 from lambdipy_b200 import strip as S  # noqa: E402
 from lambdipy_b200.device import DeviceBatch  # noqa: E402
@@ -71,7 +72,9 @@ def main():
     nproc = os.cpu_count()
     base = tempfile.mkdtemp(prefix="lb2_cfg_", dir="/dev/shm")
     ctx = N.Context(0)
-    res = {"nproc": nproc, "strip": subprocess.run(["strip", "--version"], capture_output=True, text=True).stdout.splitlines()[0], "trees": {}}
+    peak, peak_src = peaks()
+    res = {"nproc": nproc, "strip": subprocess.run(["strip", "--version"], capture_output=True, text=True).stdout.splitlines()[0],
+           "hbm_copy_gbs": peak, "hbm_copy_source": peak_src, "trees": {}}
     try:
         for name, roots in TREES.items():
             master = os.path.join(base, "master")
@@ -143,7 +146,7 @@ def main():
             r["device"] = {"n_ok": st["n_ok"], "n_unsupported": st["n_unsupported"], "plan_ms": float(np.median(plan)), "compact_ms": float(np.median(comp)),
                            "step_ms_wall": float(np.median(wall)) * 1e3, "gbs_input": in_bytes / 1e9 / (float(np.median(wall))),
                            "kernels_gbs_input": in_bytes / 1e9 / ((float(np.median(plan)) + float(np.median(comp))) / 1e3),
-                           "compact_rw_gbs": alg / 1e9 / (float(np.median(comp)) / 1e3), "compact_frac_of_6485.8": alg / 1e9 / (float(np.median(comp)) / 1e3) / 6485.8,
+                           "compact_rw_gbs": alg / 1e9 / (float(np.median(comp)) / 1e3), "compact_frac": alg / 1e9 / (float(np.median(comp)) / 1e3) / peak,
                            "copy_bytes": st["copy_bytes"], "out_bytes": st["out_bytes"], "header_bytes": st["header_bytes"]}
             b.close()
             # ---- host buffers

@@ -1,6 +1,6 @@
 // pcie_probe.cu -- what the host link gives this GPU, to choose the host-buffer pipeline (DESIGN.md section 6):
 // SM loads/stores on mapped pinned memory (the zero-copy path) vs copy-engine DMA (the staged path), each
-// direction alone and both at once.  nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/pcie_probe tools/pcie_probe.cu
+// direction alone and both at once.  nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/pcie_probe tools/pcie_probe.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -28,7 +28,9 @@ int main(int argc, char **argv) {
   CK(cudaStreamCreate(&s1)); CK(cudaStreamCreate(&s2));
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-  const int grids[] = {148, 148 * 4, 148 * 16};
+  int sms = 0;
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+  const int grids[] = {sms, sms * 4, sms * 16};
   auto timeit = [&](const char *name, auto fn, double gb_each_way, int ways) {
     fn(); cudaDeviceSynchronize();
     float best = 1e9;
@@ -51,7 +53,7 @@ int main(int argc, char **argv) {
   timeit("DMA H2D", [&] { cudaMemcpyAsync(dA, hA, bytes, cudaMemcpyHostToDevice, s1); }, gb, 1);
   timeit("DMA D2H", [&] { cudaMemcpyAsync(hB, dB, bytes, cudaMemcpyDeviceToHost, s1); }, gb, 1);
   timeit("DMA H2D + D2H", [&] { cudaMemcpyAsync(dA, hA, bytes, cudaMemcpyHostToDevice, s1); cudaMemcpyAsync(hB, dB, bytes, cudaMemcpyDeviceToHost, s2); }, gb, 2);
-  timeit("SM up + DMA down", [&] { k_copy<<<148 * 4, 256, 0, s1>>>(dA, hA, n); cudaMemcpyAsync(hB, dB, bytes, cudaMemcpyDeviceToHost, s2); }, gb, 2);
-  timeit("DMA up + SM down", [&] { cudaMemcpyAsync(dA, hA, bytes, cudaMemcpyHostToDevice, s1); k_copy<<<148 * 4, 256, 0, s2>>>(hB, dB, n); }, gb, 2);
+  timeit("SM up + DMA down", [&] { k_copy<<<sms * 4, 256, 0, s1>>>(dA, hA, n); cudaMemcpyAsync(hB, dB, bytes, cudaMemcpyDeviceToHost, s2); }, gb, 2);
+  timeit("DMA up + SM down", [&] { cudaMemcpyAsync(dA, hA, bytes, cudaMemcpyHostToDevice, s1); k_copy<<<sms * 4, 256, 0, s2>>>(hB, dB, n); }, gb, 2);
   return 0;
 }
