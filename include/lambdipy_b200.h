@@ -205,6 +205,43 @@ int lb2_corpus_fill(lb2_ctx *ctx, void *d_arena, const lb2_fill_region *h_region
 int lb2_corpus_scatter(lb2_ctx *ctx, void *d_arena, const void *h_data, uint64_t data_bytes, const uint64_t *h_dst,
                        const uint64_t *h_src, const uint64_t *h_len, uint32_t n);
 
+/* ---- gzip writer: raw DEFLATE (RFC 1951) + CRC-32 of a stream fed in pieces ----------------- */
+/* What `tarfile.open(path, "w:gz")` spends its time on in PackageBuild.create_compressed_tarball
+ * (lambdipy/package_build.py:165-172 of the reference).  The caller writes the gzip header and the
+ * CRC32 / ISIZE trailer; the library produces the DEFLATE body between them.
+ *
+ * Each piece is cut into 64 KB chunks that are deflated independently on the GPU, each looking back
+ * 32 KB into the stream (also into earlier pieces), and each ending byte-aligned with an empty stored
+ * block (what zlib's Z_SYNC_FLUSH emits).  A chunk is written with dynamic Huffman, fixed Huffman or
+ * stored blocks, whichever is smallest, so incompressible data grows by at most LB2_GZIP_BOUND.
+ * The same stream always gives the same bytes.
+ *
+ * Up to TWO pieces may be in flight: lb2_gzip_submit enqueues the upload and the kernels and returns;
+ * lb2_gzip_collect waits for the OLDEST piece and copies its compressed bytes out.  h_in must stay
+ * unchanged until its piece is collected (pinned memory from lb2_pinned_alloc makes the upload
+ * asynchronous).  lb2_gzip_finish appends the final empty block once every piece is collected.
+ * Destroy the writer before its context. */
+typedef struct lb2_gzip lb2_gzip;
+typedef struct lb2_gzip_stats {
+  uint64_t in_bytes, out_bytes;      /* stream bytes in; DEFLATE bytes out (final block included)   */
+  uint32_t crc32;                    /* CRC-32 of the input collected so far                          */
+  uint32_t n_chunks, n_stored_chunks, n_fixed_chunks;  /* 64 KB chunks; those written stored / fixed Huffman */
+  float deflate_ms;                  /* deflate + compaction kernels, CUDA events, summed over pieces */
+  float crc_ms;                      /* CRC-32 kernel                                                 */
+  float h2d_ms;                      /* piece uploads (CUDA events)                                   */
+  float d2h_ms;                      /* result downloads (host clock around the copy)                 */
+} lb2_gzip_stats;
+/* worst-case DEFLATE bytes of one piece of n input bytes (out_cap of lb2_gzip_collect) */
+#define LB2_GZIP_BOUND(n) ((n) + 15 * (((n) + 65535) / 65536))
+int lb2_gzip_create(lb2_ctx *ctx, uint32_t flags /* 0 */, lb2_gzip **g);
+int lb2_gzip_submit(lb2_gzip *g, const void *h_in, uint64_t n);
+/* LB2_E_CAPACITY when out_cap is too small: *out_n says how much is needed, the piece stays in flight */
+int lb2_gzip_collect(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n);
+/* writes the final block (2 bytes); *crc32 / *isize (full length; gzip stores it mod 2^32) for the trailer */
+int lb2_gzip_finish(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n, uint32_t *crc32, uint64_t *isize,
+                    lb2_gzip_stats *stats);
+void lb2_gzip_destroy(lb2_gzip *g);
+
 #ifdef __cplusplus
 }
 #endif

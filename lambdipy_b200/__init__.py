@@ -5,6 +5,8 @@ Public surface:
                                                 (/root/reference/lambdipy/project_build.py:260)
     strip_buffers(ctx, [bytes, ...])            same operation on in-memory ELF images
     project_build.install_non_resolved_requirements   mirror of the reference entry point
+    gzip_tarball(src_paths, tarball_path)       tar.gz of a package tree, DEFLATE on the GPU
+    tarball.create_compressed_tarball           mirror of PackageBuild.create_compressed_tarball
     patch.apply()                               monkey-patch an installed lambdipy in place
 The byte work is done by liblambdipy_b200.so (CUDA, C ABI in include/lambdipy_b200.h).
 """
@@ -15,4 +17,7 @@ def __getattr__(name):
     if name in ("strip_tree", "strip_buffers"):
         from . import strip
         return getattr(strip, name)
+    if name == "gzip_tarball":
+        from . import tarball
+        return tarball.gzip_tarball
     raise AttributeError(name)

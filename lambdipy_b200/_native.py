@@ -24,7 +24,13 @@ EXPORTS = [
     "lb2_strip_device_async", "lb2_batch_results", "lb2_strip_host", "lb2_strip_tree",
     "lb2_plan_device", "lb2_corpus_fill", "lb2_corpus_scatter",
     "lb2_strip_device_chunked", "lb2_tree_prepare", "lb2_strip_tree_ex", "lb2_tree_cleanup",
+    "lb2_gzip_create", "lb2_gzip_submit", "lb2_gzip_collect", "lb2_gzip_finish", "lb2_gzip_destroy",
 ]
+
+
+def gzip_bound(n):
+    """worst-case DEFLATE bytes of one gzip piece of n input bytes (LB2_GZIP_BOUND)"""
+    return n + 15 * ((n + 65535) // 65536)
 
 
 class Stats(C.Structure):
@@ -54,6 +60,17 @@ class TreeStats(C.Structure):
         d = {k: getattr(self, k) for k, _ in self._fields_ if k != "batch"}
         d["batch"] = self.batch.as_dict()
         return d
+
+
+class GzipStats(C.Structure):
+    _fields_ = [
+        ("in_bytes", C.c_uint64), ("out_bytes", C.c_uint64), ("crc32", C.c_uint32), ("n_chunks", C.c_uint32),
+        ("n_stored_chunks", C.c_uint32), ("n_fixed_chunks", C.c_uint32), ("deflate_ms", C.c_float), ("crc_ms", C.c_float), ("h2d_ms", C.c_float),
+        ("d2h_ms", C.c_float),
+    ]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
 
 
 class FillRegion(C.Structure):
@@ -130,6 +147,16 @@ def load():
     lib.lb2_tree_cleanup.restype = C.c_int
     lib.lb2_tree_prepare.argtypes = [vp, C.c_uint64]
     lib.lb2_tree_prepare.restype = C.c_int
+    lib.lb2_gzip_create.argtypes = [vp, C.c_uint32, C.POINTER(vp)]
+    lib.lb2_gzip_create.restype = C.c_int
+    lib.lb2_gzip_submit.argtypes = [vp, vp, C.c_uint64]
+    lib.lb2_gzip_submit.restype = C.c_int
+    lib.lb2_gzip_collect.argtypes = [vp, vp, C.c_uint64, u64p]
+    lib.lb2_gzip_collect.restype = C.c_int
+    lib.lb2_gzip_finish.argtypes = [vp, vp, C.c_uint64, u64p, C.POINTER(C.c_uint32), u64p, C.POINTER(GzipStats)]
+    lib.lb2_gzip_finish.restype = C.c_int
+    lib.lb2_gzip_destroy.argtypes = [vp]
+    lib.lb2_gzip_destroy.restype = None
     _lib = lib
     return lib
 

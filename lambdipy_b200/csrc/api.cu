@@ -1450,3 +1450,192 @@ int lb2_corpus_scatter(lb2_ctx *ctx, void *d_arena, const void *h_data, uint64_t
 }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------------------- gzip writer
+// Device buffers of one piece in flight.  d_in holds GZ_HIST bytes of history in front of the piece: the tail of
+// the stream so far, copied there from lb2_gzip::d_hist, so every chunk can look back 32 KB across piece boundaries.
+struct GzSlot {
+  uint8_t *d_in = nullptr, *d_chunk_out = nullptr, *d_out = nullptr;
+  uint32_t *d_tok = nullptr, *d_meta = nullptr;  // meta: size | mode | crc, n_chunks each
+  uint64_t *d_off = nullptr;
+  GzResult *d_res = nullptr, *h_res = nullptr;
+  uint32_t cap_chunks = 0;
+  cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // upload | deflate | crc | compact |
+  cudaEvent_t done = nullptr;
+  uint64_t n = 0;
+};
+
+struct lb2_gzip {
+  lb2_ctx *ctx = nullptr;
+  cudaStream_t stream = nullptr;
+  uint8_t *d_hist = nullptr;   // last <= GZ_HIST bytes of the stream
+  uint32_t *d_crc = nullptr;   // running CRC-32, advanced by each piece's scan kernel
+  uint64_t hist_len = 0;
+  GzSlot slot[2];
+  int head = 0, count = 0;     // pieces in flight, collected in submission order
+  bool finished = false;
+  lb2_gzip_stats st{};
+};
+
+static void gz_slot_free(GzSlot &s) {
+  cudaFree(s.d_in); cudaFree(s.d_chunk_out); cudaFree(s.d_out); cudaFree(s.d_tok); cudaFree(s.d_meta); cudaFree(s.d_off);
+  cudaFree(s.d_res);
+  if (s.h_res) cudaFreeHost(s.h_res);
+  for (auto &e : s.ev) if (e) cudaEventDestroy(e);
+  if (s.done) cudaEventDestroy(s.done);
+  s = GzSlot();
+}
+
+static int gz_slot_reserve(lb2_ctx *ctx, GzSlot &s, uint32_t n_chunks) {
+  if (!s.d_res) {
+    CK(cudaMalloc(&s.d_res, sizeof(GzResult)));
+    CK(cudaHostAlloc(&s.h_res, sizeof(GzResult), cudaHostAllocDefault));
+    for (auto &e : s.ev) CK(cudaEventCreate(&e));
+    CK(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
+  }
+  if (n_chunks <= s.cap_chunks) return LB2_OK;
+  cudaFree(s.d_in); cudaFree(s.d_chunk_out); cudaFree(s.d_out); cudaFree(s.d_tok); cudaFree(s.d_meta); cudaFree(s.d_off);
+  s.d_in = s.d_chunk_out = s.d_out = nullptr; s.d_tok = s.d_meta = nullptr; s.d_off = nullptr;
+  s.cap_chunks = 0;
+  const uint64_t n = n_chunks;
+  CK(cudaMalloc(&s.d_in, GZ_HIST + n * GZ_CHUNK + 16));
+  CK(cudaMalloc(&s.d_chunk_out, n * GZ_CHUNK_OUT_CAP));
+  CK(cudaMalloc(&s.d_out, n * (GZ_CHUNK + 15) + 16));
+  CK(cudaMalloc(&s.d_tok, n * GZ_CHUNK * sizeof(uint32_t)));
+  CK(cudaMalloc(&s.d_meta, 3 * n * sizeof(uint32_t)));
+  CK(cudaMalloc(&s.d_off, n * sizeof(uint64_t)));
+  s.cap_chunks = n_chunks;
+  return LB2_OK;
+}
+
+extern "C" {
+
+int lb2_gzip_create(lb2_ctx *ctx, uint32_t flags, lb2_gzip **out) {
+  if (!ctx || !out) { if (ctx) ctx->err = "NULL argument"; return LB2_E_ARG; }
+  *out = nullptr;
+  if (flags) { ctx->err = "lb2_gzip_create: no flags are defined"; return LB2_E_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  lb2_gzip *g = new lb2_gzip();
+  g->ctx = ctx;
+  cudaError_t e;
+  if ((e = cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking)) != cudaSuccess ||
+      (e = cudaMalloc(&g->d_hist, GZ_HIST)) != cudaSuccess || (e = cudaMalloc(&g->d_crc, sizeof(uint32_t))) != cudaSuccess ||
+      (e = cudaMemsetAsync(g->d_crc, 0, sizeof(uint32_t), g->stream)) != cudaSuccess) {
+    ctx->err = std::string("lb2_gzip_create: ") + cudaGetErrorString(e);
+    lb2_gzip_destroy(g);
+    return LB2_E_CUDA;
+  }
+  *out = g;
+  return LB2_OK;
+}
+
+void lb2_gzip_destroy(lb2_gzip *g) {
+  if (!g) return;
+  cudaSetDevice(g->ctx->device);
+  if (g->stream) cudaStreamSynchronize(g->stream);
+  for (auto &s : g->slot) gz_slot_free(s);
+  cudaFree(g->d_hist);
+  cudaFree(g->d_crc);
+  if (g->stream) cudaStreamDestroy(g->stream);
+  delete g;
+}
+
+int lb2_gzip_submit(lb2_gzip *g, const void *h_in, uint64_t n) {
+  if (!g) return LB2_E_ARG;
+  lb2_ctx *ctx = g->ctx;
+  if (!h_in && n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if (g->finished) { ctx->err = "lb2_gzip_submit after lb2_gzip_finish"; return LB2_E_STATE; }
+  if (g->count >= 2) { ctx->err = "two pieces already in flight: collect one with lb2_gzip_collect first"; return LB2_E_STATE; }
+  if (n > (uint64_t)UINT32_MAX * GZ_CHUNK / 2) { ctx->err = "piece too large"; return LB2_E_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  GzSlot &s = g->slot[(g->head + g->count) & 1];
+  s.n = n;
+  if (n) {
+    const uint32_t n_chunks = (uint32_t)((n + GZ_CHUNK - 1) / GZ_CHUNK);
+    int rc = gz_slot_reserve(ctx, s, n_chunks);
+    if (rc) return rc;
+    cudaStream_t st = g->stream;
+    GzPieceArgs a;
+    a.in = s.d_in + GZ_HIST; a.n = n; a.hist = (uint32_t)g->hist_len; a.n_chunks = n_chunks;
+    a.tokens = s.d_tok; a.chunk_out = s.d_chunk_out;
+    a.chunk_size = s.d_meta; a.chunk_mode = s.d_meta + n_chunks; a.chunk_crc = s.d_meta + 2 * n_chunks;
+    a.chunk_off = s.d_off; a.out = s.d_out; a.crc_state = g->d_crc; a.res = s.d_res;
+    CK(cudaEventRecord(s.ev[0], st));
+    if (g->hist_len)
+      CK(cudaMemcpyAsync(s.d_in + GZ_HIST - g->hist_len, g->d_hist, g->hist_len, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(s.d_in + GZ_HIST, h_in, n, cudaMemcpyHostToDevice, st));
+    CK(cudaEventRecord(s.ev[1], st));
+    launch_deflate(a, st);
+    CK(cudaEventRecord(s.ev[2], st));
+    launch_crc32(a, st);
+    CK(cudaEventRecord(s.ev[3], st));
+    launch_gzip_compact(a, st);
+    CK(cudaEventRecord(s.ev[4], st));
+    CK(cudaMemcpyAsync(s.h_res, s.d_res, sizeof(GzResult), cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(s.done, st));
+    // history of the next piece: the stream's last <= 32 KB, which end with this piece
+    const uint64_t keep = std::min<uint64_t>(GZ_HIST, g->hist_len + n);
+    CK(cudaMemcpyAsync(g->d_hist, s.d_in + GZ_HIST + n - keep, keep, cudaMemcpyDeviceToDevice, st));
+    CK(cudaGetLastError());
+    g->hist_len = keep;
+    g->st.n_chunks += n_chunks;
+  }
+  g->st.in_bytes += n;
+  g->count++;
+  return LB2_OK;
+}
+
+int lb2_gzip_collect(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n) {
+  if (!g) return LB2_E_ARG;
+  lb2_ctx *ctx = g->ctx;
+  if (!out_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if (!g->count) { ctx->err = "no piece in flight"; return LB2_E_STATE; }
+  CK(cudaSetDevice(ctx->device));
+  GzSlot &s = g->slot[g->head];
+  uint64_t total = 0;
+  if (s.n) {
+    CK(cudaEventSynchronize(s.done));
+    total = s.h_res->out_bytes;
+    *out_n = total;
+    if (total > out_cap) { ctx->err = "output buffer too small for this piece (*out_n bytes needed)"; return LB2_E_CAPACITY; }
+    if (!h_out) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+    const double t0 = now_s();
+    CK(cudaMemcpy(h_out, s.d_out, total, cudaMemcpyDeviceToHost));
+    g->st.d2h_ms += (float)((now_s() - t0) * 1e3);
+    float ms = 0;
+    CK(cudaEventElapsedTime(&ms, s.ev[0], s.ev[1])); g->st.h2d_ms += ms;
+    CK(cudaEventElapsedTime(&ms, s.ev[1], s.ev[2])); g->st.deflate_ms += ms;
+    CK(cudaEventElapsedTime(&ms, s.ev[3], s.ev[4])); g->st.deflate_ms += ms;
+    CK(cudaEventElapsedTime(&ms, s.ev[2], s.ev[3])); g->st.crc_ms += ms;
+    g->st.crc32 = s.h_res->crc32;
+    g->st.n_stored_chunks += s.h_res->n_stored;
+    g->st.n_fixed_chunks += s.h_res->n_fixed;
+    g->st.out_bytes += total;
+  }
+  *out_n = total;
+  g->head ^= 1;
+  g->count--;
+  return LB2_OK;
+}
+
+int lb2_gzip_finish(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n, uint32_t *crc32, uint64_t *isize,
+                    lb2_gzip_stats *stats) {
+  if (!g) return LB2_E_ARG;
+  lb2_ctx *ctx = g->ctx;
+  if (!h_out || !out_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if (g->count) { ctx->err = "pieces still in flight: collect them first"; return LB2_E_STATE; }
+  if (g->finished) { ctx->err = "lb2_gzip_finish called twice"; return LB2_E_STATE; }
+  *out_n = 2;
+  if (out_cap < 2) { ctx->err = "output buffer too small"; return LB2_E_CAPACITY; }
+  // final block: BFINAL 1, fixed Huffman, end-of-block code -- the two bytes zlib ends a flushed stream with
+  static_cast<uint8_t *>(h_out)[0] = 0x03;
+  static_cast<uint8_t *>(h_out)[1] = 0x00;
+  g->finished = true;
+  g->st.out_bytes += 2;
+  if (crc32) *crc32 = g->st.crc32;
+  if (isize) *isize = g->st.in_bytes;
+  if (stats) *stats = g->st;
+  return LB2_OK;
+}
+
+}  // extern "C"
