@@ -44,10 +44,12 @@ enum {
   LB2_OK = 0,
   LB2_E_CUDA = -1,        /* CUDA runtime error; text in lb2_last_error */
   LB2_E_ARG = -2,         /* bad argument (NULL, unaligned offsets, ...) */
-  LB2_E_CAPACITY = -3,    /* output arena too small; stats.out_bytes_needed says how much */
+  LB2_E_CAPACITY = -3,    /* output arena too small (stats.out_bytes_needed says how much); lb2_inflate_run: the
+                             stream does not fit in device memory */
   LB2_E_IO = -4,          /* filesystem error in lb2_strip_tree */
   LB2_E_NODEVICE = -5,    /* no usable CUDA device */
-  LB2_E_STATE = -6        /* call out of order (no batch in flight, ...) */
+  LB2_E_STATE = -6,       /* call out of order (no batch in flight, ...) */
+  LB2_E_DATA = -7         /* lb2_inflate_run: the DEFLATE stream is invalid or truncated */
 };
 
 /* per-file status written by the plan kernel */
@@ -241,6 +243,37 @@ int lb2_gzip_collect(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n
 int lb2_gzip_finish(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n, uint32_t *crc32, uint64_t *isize,
                     lb2_gzip_stats *stats);
 void lb2_gzip_destroy(lb2_gzip *g);
+
+/* ---- gzip reader: raw DEFLATE (RFC 1951) decoded on the GPU ----------------------------------- */
+/* What `tarfile.open(path, "r:gz")` spends its time on in prepare_tarfile (lambdipy/project_build.py:98-102 of the
+ * reference).  The caller parses the gzip header and trailer; the library decodes the DEFLATE body in between.
+ *
+ * Any valid stream decodes, also one with no flush points: the body is cut into spans of LB2_INFLATE_SPAN_KB (read
+ * at each call, default 128) compressed KB; each span after the first starts at a block-header candidate found by
+ * search, is decoded speculatively, and is used only if its start is where the span before it ended (otherwise it
+ * is decoded again from that confirmed position).  Invalid or truncated input gives LB2_E_DATA, never other bytes.
+ * Device memory: the body plus about 3 bytes per decoded byte (LB2_E_CAPACITY when that does not fit).
+ *
+ * lb2_inflate_run decodes the stream that starts at h_in; bytes after its final block (a gzip trailer, further
+ * members) are ignored, and stats.in_bytes says where the stream ended.  The decoded bytes stay on the device until
+ * lb2_inflate_read copies them out (the next run replaces them).  Destroy the reader before its context. */
+typedef struct lb2_inflate lb2_inflate;
+typedef struct lb2_inflate_stats {
+  uint64_t in_bytes, out_bytes;   /* DEFLATE bytes consumed (to the end of the final block), bytes produced       */
+  uint32_t crc32;                 /* CRC-32 of the decoded bytes                                                  */
+  uint32_t n_spans;               /* spans decoded on their own                                                   */
+  uint32_t n_rounds;              /* count rounds of the chain                                                    */
+  uint32_t n_rejected;            /* candidates the chain rejected (a wrong start, decoded again from the right one) */
+  uint32_t n_absorbed;            /* nominal spans without a candidate, decoded by the span before them          */
+  float find_ms, count_ms, decode_ms, resolve_ms, crc_ms;  /* kernel times (CUDA events), count summed over rounds */
+  float h2d_ms;                   /* body upload (CUDA events)                                                    */
+} lb2_inflate_stats;
+int lb2_inflate_create(lb2_ctx *ctx, uint32_t flags /* 0 */, lb2_inflate **d);
+/* decode the raw DEFLATE stream at h_in (at most n bytes) on the device; *out_n = its exact decoded size */
+int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_n, lb2_inflate_stats *stats);
+/* copy the decoded bytes of the last successful run to h_out (cap >= *out_n) */
+int lb2_inflate_read(lb2_inflate *d, void *h_out, uint64_t cap);
+void lb2_inflate_destroy(lb2_inflate *d);
 
 #ifdef __cplusplus
 }

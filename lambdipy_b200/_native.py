@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("LAMBDIPY_B200_LIB") or os.path.join(_HERE, "liblambdipy_b200.so")  # (override: diagnostic builds)
 
 # return codes / status / flags (mirror include/lambdipy_b200.h)
-LB2_OK, LB2_E_CUDA, LB2_E_ARG, LB2_E_CAPACITY, LB2_E_IO, LB2_E_NODEVICE, LB2_E_STATE = 0, -1, -2, -3, -4, -5, -6
+LB2_OK, LB2_E_CUDA, LB2_E_ARG, LB2_E_CAPACITY, LB2_E_IO, LB2_E_NODEVICE, LB2_E_STATE, LB2_E_DATA = 0, -1, -2, -3, -4, -5, -6, -7
 ST_OK, ST_NOT_ELF, ST_NOT_ELF64LE, ST_BAD_TYPE, ST_NO_SECTIONS, ST_XINDEX = 0, 1, 2, 3, 4, 5
 ST_UNSUPPORTED_LAYOUT, ST_BAD_NOTES, ST_PLANNER_LIMIT, ST_MALFORMED = 6, 7, 8, -1
 F_NO_MERGE_NOTES = 1
@@ -25,6 +25,7 @@ EXPORTS = [
     "lb2_plan_device", "lb2_corpus_fill", "lb2_corpus_scatter",
     "lb2_strip_device_chunked", "lb2_tree_prepare", "lb2_strip_tree_ex", "lb2_tree_cleanup",
     "lb2_gzip_create", "lb2_gzip_submit", "lb2_gzip_collect", "lb2_gzip_finish", "lb2_gzip_destroy",
+    "lb2_inflate_create", "lb2_inflate_run", "lb2_inflate_read", "lb2_inflate_destroy",
 ]
 
 
@@ -67,6 +68,18 @@ class GzipStats(C.Structure):
         ("in_bytes", C.c_uint64), ("out_bytes", C.c_uint64), ("crc32", C.c_uint32), ("n_chunks", C.c_uint32),
         ("n_stored_chunks", C.c_uint32), ("n_fixed_chunks", C.c_uint32), ("deflate_ms", C.c_float), ("crc_ms", C.c_float), ("h2d_ms", C.c_float),
         ("d2h_ms", C.c_float),
+    ]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class InflateStats(C.Structure):
+    _fields_ = [
+        ("in_bytes", C.c_uint64), ("out_bytes", C.c_uint64), ("crc32", C.c_uint32), ("n_spans", C.c_uint32),
+        ("n_rounds", C.c_uint32), ("n_rejected", C.c_uint32), ("n_absorbed", C.c_uint32),
+        ("find_ms", C.c_float), ("count_ms", C.c_float), ("decode_ms", C.c_float), ("resolve_ms", C.c_float),
+        ("crc_ms", C.c_float), ("h2d_ms", C.c_float),
     ]
 
     def as_dict(self):
@@ -157,6 +170,14 @@ def load():
     lib.lb2_gzip_finish.restype = C.c_int
     lib.lb2_gzip_destroy.argtypes = [vp]
     lib.lb2_gzip_destroy.restype = None
+    lib.lb2_inflate_create.argtypes = [vp, C.c_uint32, C.POINTER(vp)]
+    lib.lb2_inflate_create.restype = C.c_int
+    lib.lb2_inflate_run.argtypes = [vp, vp, C.c_uint64, u64p, C.POINTER(InflateStats)]
+    lib.lb2_inflate_run.restype = C.c_int
+    lib.lb2_inflate_read.argtypes = [vp, vp, C.c_uint64]
+    lib.lb2_inflate_read.restype = C.c_int
+    lib.lb2_inflate_destroy.argtypes = [vp]
+    lib.lb2_inflate_destroy.restype = None
     _lib = lib
     return lib
 

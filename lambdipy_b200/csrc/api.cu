@@ -1639,3 +1639,202 @@ int lb2_gzip_finish(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n,
 }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------------------- gzip reader
+// Speculative parallel inflate (inflate_core.cuh, kernels in inflate.cu).  The body is uploaded once; candidate
+// search, count rounds (the chain runs here on the host between rounds), decode, resolve and CRC-32 run on the
+// reader's stream; the decoded bytes stay on the device until lb2_inflate_read.
+#include "inflate_core.cuh"
+
+struct lb2_inflate {
+  lb2_ctx *ctx = nullptr;
+  cudaStream_t stream = nullptr;
+  uint8_t *d_in = nullptr, *d_out = nullptr;
+  uint16_t *d_arena = nullptr;
+  uint64_t *d_cand = nullptr;
+  ifl::SpanJob *d_jobs = nullptr;
+  ifl::SpanResult *d_res = nullptr;
+  uint32_t *d_chunk_crc = nullptr, *d_crc = nullptr;
+  int32_t *d_err = nullptr;
+  uint64_t cap_in = 0, cap_cand = 0, cap_jobs = 0, cap_res = 0, cap_arena = 0, cap_out = 0, cap_chunks = 0;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  uint64_t out_n = 0;
+  bool have = false;
+};
+
+// (re)allocates *p for `need` bytes when `cap` is smaller; LB2_E_CAPACITY when the device has no room
+template <class T> static int ifl_grow(lb2_ctx *ctx, T **p, uint64_t &cap, uint64_t need, size_t elem) {
+  if (need <= cap) return LB2_OK;
+  cudaFree(*p);
+  *p = nullptr;
+  cap = 0;
+  const cudaError_t e = cudaMalloc(p, need * elem + 16);
+  if (e == cudaErrorMemoryAllocation) {
+    cudaGetLastError();
+    ctx->err = "lb2_inflate_run: the stream does not fit in device memory";
+    return LB2_E_CAPACITY;
+  }
+  CK(e);
+  cap = need;
+  return LB2_OK;
+}
+
+static float ifl_elapsed(lb2_inflate *d) {
+  float ms = 0;
+  cudaEventElapsedTime(&ms, d->ev[0], d->ev[1]);
+  return ms;
+}
+
+extern "C" {
+
+int lb2_inflate_create(lb2_ctx *ctx, uint32_t flags, lb2_inflate **out) {
+  if (!ctx || !out) { if (ctx) ctx->err = "NULL argument"; return LB2_E_ARG; }
+  *out = nullptr;
+  if (flags) { ctx->err = "lb2_inflate_create: no flags are defined"; return LB2_E_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  lb2_inflate *d = new lb2_inflate();
+  d->ctx = ctx;
+  cudaError_t e;
+  if ((e = cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking)) != cudaSuccess ||
+      (e = cudaEventCreate(&d->ev[0])) != cudaSuccess || (e = cudaEventCreate(&d->ev[1])) != cudaSuccess ||
+      (e = cudaMalloc(&d->d_crc, sizeof(uint32_t))) != cudaSuccess || (e = cudaMalloc(&d->d_err, sizeof(int32_t))) != cudaSuccess) {
+    ctx->err = std::string("lb2_inflate_create: ") + cudaGetErrorString(e);
+    lb2_inflate_destroy(d);
+    return LB2_E_CUDA;
+  }
+  *out = d;
+  return LB2_OK;
+}
+
+void lb2_inflate_destroy(lb2_inflate *d) {
+  if (!d) return;
+  cudaSetDevice(d->ctx->device);
+  if (d->stream) cudaStreamSynchronize(d->stream);
+  cudaFree(d->d_in); cudaFree(d->d_out); cudaFree(d->d_arena); cudaFree(d->d_cand); cudaFree(d->d_jobs); cudaFree(d->d_res);
+  cudaFree(d->d_chunk_crc); cudaFree(d->d_crc); cudaFree(d->d_err);
+  for (auto &e : d->ev) if (e) cudaEventDestroy(e);
+  if (d->stream) cudaStreamDestroy(d->stream);
+  delete d;
+}
+
+int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_n, lb2_inflate_stats *stats) {
+  if (!d) return LB2_E_ARG;
+  lb2_ctx *ctx = d->ctx;
+  if ((!h_in && n) || !out_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  d->have = false;
+  *out_n = 0;
+  lb2_inflate_stats st{};
+  uint64_t span = 128 << 10;
+  if (const char *v = getenv("LB2_INFLATE_SPAN_KB")) {
+    const long kb = atol(v);
+    if (kb < 1) { ctx->err = "LB2_INFLATE_SPAN_KB must be a positive number of KB"; return LB2_E_ARG; }
+    span = (uint64_t)kb << 10;
+  }
+  const uint32_t n_spans = n > span ? (uint32_t)((n + span - 1) / span) : 1;
+  cudaStream_t s = d->stream;
+  int rc;
+  if ((rc = ifl_grow(ctx, &d->d_in, d->cap_in, n, 1)) || (rc = ifl_grow(ctx, &d->d_cand, d->cap_cand, n_spans, sizeof(uint64_t))) ||
+      (rc = ifl_grow(ctx, &d->d_jobs, d->cap_jobs, n_spans, sizeof(ifl::SpanJob))) ||
+      (rc = ifl_grow(ctx, &d->d_res, d->cap_res, n_spans, sizeof(ifl::SpanResult))))
+    return rc;
+  // upload
+  CK(cudaEventRecord(d->ev[0], s));
+  if (n) CK(cudaMemcpyAsync(d->d_in, h_in, n, cudaMemcpyHostToDevice, s));
+  CK(cudaEventRecord(d->ev[1], s));
+  CK(cudaEventSynchronize(d->ev[1]));
+  st.h2d_ms = ifl_elapsed(d);
+  // candidates
+  std::vector<uint64_t> cand(n_spans, ifl::KEY_NONE);
+  CK(cudaEventRecord(d->ev[0], s));
+  launch_inflate_find(d->d_in, n, span, n_spans, d->d_cand, s);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(d->ev[1], s));
+  if (n_spans > 1) CK(cudaMemcpyAsync(cand.data() + 1, d->d_cand + 1, (n_spans - 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  st.find_ms = ifl_elapsed(d);
+  // count rounds and chain
+  ifl::Chain c;
+  c.init(cand.data(), n_spans, span, n, ifl::GIVE_UP_SPANS);
+  std::vector<ifl::SpanJob> jobs;
+  std::vector<ifl::SpanResult> res;
+  while (!c.done && !c.error) {
+    const std::vector<uint32_t> p = c.pending();
+    jobs.resize(p.size());
+    res.resize(p.size());
+    for (size_t i = 0; i < p.size(); i++) jobs[i] = c.job[p[i]];
+    CK(cudaMemcpyAsync(d->d_jobs, jobs.data(), jobs.size() * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(d->ev[0], s));
+    launch_inflate_count(d->d_in, n, d->d_jobs, (uint32_t)jobs.size(), d->d_res, s);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(d->ev[1], s));
+    CK(cudaMemcpyAsync(res.data(), d->d_res, res.size() * sizeof(ifl::SpanResult), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    st.count_ms += ifl_elapsed(d);
+    for (size_t i = 0; i < p.size(); i++) c.set_result(p[i], res[i]);
+    c.advance();
+  }
+  st.n_rounds = c.n_rounds;
+  st.n_rejected = c.n_rejected;
+  st.n_absorbed = c.n_absorbed;
+  if (c.error) {
+    ctx->err = "lb2_inflate_run: invalid DEFLATE stream (span status " + std::to_string(c.error) + ")";
+    if (stats) *stats = st;
+    return LB2_E_DATA;
+  }
+  const uint64_t total = c.layout();
+  const uint32_t n_used = (uint32_t)c.job.size();
+  st.n_spans = n_used;
+  st.in_bytes = c.in_bytes();
+  st.out_bytes = total;
+  // 2 bytes per output byte for the u16 arena, 1 for the final bytes
+  if ((rc = ifl_grow(ctx, &d->d_arena, d->cap_arena, total, sizeof(uint16_t))) || (rc = ifl_grow(ctx, &d->d_out, d->cap_out, total, 1)) ||
+      (rc = ifl_grow(ctx, &d->d_chunk_crc, d->cap_chunks, (total + GZ_CHUNK - 1) / GZ_CHUNK + 1, sizeof(uint32_t))))
+    return rc;
+  // decode, resolve, CRC-32
+  CK(cudaMemcpyAsync(d->d_jobs, c.job.data(), n_used * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(d->d_err, 0, sizeof(int32_t), s));
+  CK(cudaEventRecord(d->ev[0], s));
+  launch_inflate_decode(d->d_in, n, d->d_jobs, n_used, d->d_arena, d->d_err, s);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(d->ev[1], s));
+  CK(cudaEventSynchronize(d->ev[1]));
+  st.decode_ms = ifl_elapsed(d);
+  CK(cudaEventRecord(d->ev[0], s));
+  launch_inflate_resolve(d->d_arena, d->d_out, d->d_jobs, n_used, d->d_err, s);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(d->ev[1], s));
+  CK(cudaEventSynchronize(d->ev[1]));
+  st.resolve_ms = ifl_elapsed(d);
+  CK(cudaEventRecord(d->ev[0], s));
+  launch_crc32(d->d_out, total, d->d_chunk_crc, d->d_crc, s);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(d->ev[1], s));
+  int32_t err = 0;
+  CK(cudaMemcpyAsync(&st.crc32, d->d_crc, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&err, d->d_err, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  st.crc_ms = ifl_elapsed(d);
+  if (stats) *stats = st;
+  if (err) {
+    ctx->err = "lb2_inflate_run: invalid DEFLATE stream (decode status " + std::to_string(err) + ")";
+    return LB2_E_DATA;
+  }
+  d->out_n = total;
+  d->have = true;
+  *out_n = total;
+  return LB2_OK;
+}
+
+int lb2_inflate_read(lb2_inflate *d, void *h_out, uint64_t cap) {
+  if (!d) return LB2_E_ARG;
+  lb2_ctx *ctx = d->ctx;
+  if (!d->have) { ctx->err = "lb2_inflate_read: no decoded stream (lb2_inflate_run failed or was not called)"; return LB2_E_STATE; }
+  if (cap < d->out_n) { ctx->err = "lb2_inflate_read: buffer smaller than the decoded stream"; return LB2_E_CAPACITY; }
+  if (!h_out && d->out_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  if (d->out_n) CK(cudaMemcpy(h_out, d->d_out, d->out_n, cudaMemcpyDeviceToHost));
+  return LB2_OK;
+}
+
+}  // extern "C"

@@ -525,7 +525,8 @@ __device__ uint32_t crc_combine(uint32_t crc_a, uint32_t crc_b, uint64_t len_b, 
   return multmodp(p, crc_a) ^ crc_b;
 }
 
-__global__ void __launch_bounds__(CRC_THREADS) lb2_crc32_kernel(GzPieceArgs a) {
+// CRC-32 of each GZ_CHUNK-byte chunk of in[0 .. n); in is 16-byte aligned
+__global__ void __launch_bounds__(CRC_THREADS) lb2_crc32_kernel(const uint8_t *in, uint64_t n, uint32_t *chunk_crc) {
   __shared__ uint32_t tab[256], xt[32], s_crc[CRC_THREADS], s_len[CRC_THREADS];
   const int tid = threadIdx.x;
   {
@@ -536,11 +537,11 @@ __global__ void __launch_bounds__(CRC_THREADS) lb2_crc32_kernel(GzPieceArgs a) {
   if (tid == 0) init_x2n(xt);
   __syncthreads();
   const uint64_t c0 = (uint64_t)blockIdx.x * GZ_CHUNK + (uint64_t)tid * CRC_SUB;
-  const uint32_t len = c0 >= a.n ? 0 : (uint32_t)(a.n - c0 < CRC_SUB ? a.n - c0 : CRC_SUB);
-  const uint8_t *p = a.in + c0;
+  const uint32_t len = c0 >= n ? 0 : (uint32_t)(n - c0 < CRC_SUB ? n - c0 : CRC_SUB);
+  const uint8_t *p = in + c0;
   uint32_t crc = 0xFFFFFFFFu;
   uint32_t i = 0;
-  for (; i + 16 <= len; i += 16) {  // piece data starts 16-aligned (api.cu), sub-blocks are multiples of 16
+  for (; i + 16 <= len; i += 16) {  // sub-blocks are multiples of 16
     const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p + i));
     const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
@@ -557,7 +558,7 @@ __global__ void __launch_bounds__(CRC_THREADS) lb2_crc32_kernel(GzPieceArgs a) {
     }
     __syncthreads();
   }
-  if (tid == 0) a.chunk_crc[blockIdx.x] = s_crc[0];
+  if (tid == 0) chunk_crc[blockIdx.x] = s_crc[0];
 }
 
 // ---- offsets, stream CRC, gather ---------------------------------------------------------------------------------
@@ -611,6 +612,36 @@ __global__ void __launch_bounds__(SCAN_THREADS) lb2_gzip_scan_kernel(GzPieceArgs
   }
 }
 
+// CRC-32 of a whole buffer from the per-chunk CRCs of lb2_crc32_kernel
+__global__ void __launch_bounds__(SCAN_THREADS) lb2_crc32_combine_kernel(const uint32_t *chunk_crc, uint64_t n, uint32_t *crc) {
+  __shared__ unsigned long long s_len[SCAN_THREADS];
+  __shared__ uint32_t s_crc[SCAN_THREADS], xt[32];
+  const int tid = threadIdx.x;
+  if (tid == 0) init_x2n(xt);
+  __syncthreads();
+  const uint64_t n_chunks = (n + GZ_CHUNK - 1) / GZ_CHUNK;
+  const uint64_t per = (n_chunks + SCAN_THREADS - 1) / SCAN_THREADS;
+  const uint64_t b = min(n_chunks, tid * per), e = min(n_chunks, b + per);
+  uint32_t c = 0;
+  unsigned long long len = 0;
+  for (uint64_t i = b; i < e; i++) {
+    const uint64_t cl = n - i * GZ_CHUNK < GZ_CHUNK ? n - i * GZ_CHUNK : GZ_CHUNK;
+    c = crc_combine(c, chunk_crc[i], cl, xt);
+    len += cl;
+  }
+  s_crc[tid] = c;
+  s_len[tid] = len;
+  __syncthreads();
+  for (int s = 1; s < SCAN_THREADS; s <<= 1) {
+    if ((tid & (2 * s - 1)) == 0) {
+      s_crc[tid] = crc_combine(s_crc[tid], s_crc[tid + s], s_len[tid + s], xt);
+      s_len[tid] += s_len[tid + s];
+    }
+    __syncthreads();
+  }
+  if (tid == 0) *crc = s_crc[0];
+}
+
 // one warp per chunk, with the compaction kernels' byte mover
 __global__ void __launch_bounds__(256) lb2_gzip_gather_kernel(GzPieceArgs a) {
   const uint32_t c = blockIdx.x * 8 + (threadIdx.x >> 5);
@@ -624,7 +655,15 @@ void launch_deflate(const GzPieceArgs &a, cudaStream_t s) {
   cudaFuncSetAttribute(lb2_deflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM);
   lb2_deflate_kernel<<<a.n_chunks, DF_THREADS, DF_DYN_SMEM, s>>>(a);
 }
-void launch_crc32(const GzPieceArgs &a, cudaStream_t s) { lb2_crc32_kernel<<<a.n_chunks, CRC_THREADS, 0, s>>>(a); }
+void launch_crc32(const GzPieceArgs &a, cudaStream_t s) { lb2_crc32_kernel<<<a.n_chunks, CRC_THREADS, 0, s>>>(a.in, a.n, a.chunk_crc); }
+void launch_crc32(const uint8_t *in, uint64_t n, uint32_t *chunk_crc, uint32_t *crc, cudaStream_t s) {
+  if (!n) {
+    cudaMemsetAsync(crc, 0, sizeof(uint32_t), s);
+    return;
+  }
+  lb2_crc32_kernel<<<(unsigned)((n + GZ_CHUNK - 1) / GZ_CHUNK), CRC_THREADS, 0, s>>>(in, n, chunk_crc);
+  lb2_crc32_combine_kernel<<<1, SCAN_THREADS, 0, s>>>(chunk_crc, n, crc);
+}
 void launch_gzip_compact(const GzPieceArgs &a, cudaStream_t s) {
   lb2_gzip_scan_kernel<<<1, SCAN_THREADS, 0, s>>>(a);
   lb2_gzip_gather_kernel<<<(a.n_chunks + 7) / 8, 256, 0, s>>>(a);

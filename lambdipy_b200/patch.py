@@ -8,18 +8,23 @@ its options, PackageBuild and every other function keep running the reference's 
 
 With LAMBDIPY_TARBALL_BACKEND=b200 (default: python, the reference's own code),
 PackageBuild.create_compressed_tarball is replaced as well, by the mirror in tarball.py that compresses
-on the GPU.
+on the GPU.  With LAMBDIPY_UNTAR_BACKEND=b200 (default: python), lambdipy.project_build.prepare_tarfile is
+replaced by the mirror that inflates on the GPU (download_and_prepare_asset looks the name up at call time).
 """
 import os
 import sys
 
 TARBALL_BACKENDS = ("python", "b200")
+UNTAR_BACKENDS = ("python", "b200")
 
 
 def apply():
     backend = os.environ.get("LAMBDIPY_TARBALL_BACKEND", "python")  # checked before anything is rebound
     if backend not in TARBALL_BACKENDS:
         raise ValueError("LAMBDIPY_TARBALL_BACKEND=%r: expected one of %s" % (backend, ", ".join(TARBALL_BACKENDS)))
+    untar = os.environ.get("LAMBDIPY_UNTAR_BACKEND", "python")
+    if untar not in UNTAR_BACKENDS:
+        raise ValueError("LAMBDIPY_UNTAR_BACKEND=%r: expected one of %s" % (untar, ", ".join(UNTAR_BACKENDS)))
     import lambdipy.cli as cli
     import lambdipy.project_build as ref
     from . import project_build as mine
@@ -29,6 +34,9 @@ def apply():
         import lambdipy.package_build as ref_pkg
         from . import tarball
         ref_pkg.PackageBuild.create_compressed_tarball = tarball.create_compressed_tarball
+    if untar == "b200":
+        from . import tarball
+        ref.prepare_tarfile = tarball.prepare_tarfile
     # `lambdipy build` spends seconds resolving, downloading and copying packages before it reaches the
     # strip step (cli.py:52-67): create the CUDA context behind that, not in front of the strip
     if os.environ.get("LAMBDIPY_B200_EAGER_WARMUP", "1") != "0":

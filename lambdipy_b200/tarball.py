@@ -10,14 +10,25 @@ encoder behind `lb2_gzip_*` (csrc/deflate.cu).  The result is an ordinary gzip f
     gzip_tarball(src_paths, tarball_path)          tar + gzip a list of paths, each under its basename
     create_compressed_tarball(package_build)       the reference method's mirror (patch.apply() installs it
                                                    when LAMBDIPY_TARBALL_BACKEND=b200)
+
+Reading goes the other way: `gunzip` decodes each gzip member's DEFLATE body with the CUDA decoder behind
+`lb2_inflate_*` (csrc/inflate.cu), and the standard library's `tarfile` parses and writes the tar stream.
+
+    gunzip(path)                                   the decompressed bytes of a gzip file
+    extract_tarball(tarball_path, directory)       tarfile.open(..., "r:gz").extractall(directory), inflated on the GPU
+    prepare_tarfile(url, download_filename, package_directory)
+                                                   the reference function's mirror (patch.apply() installs it
+                                                   when LAMBDIPY_UNTAR_BACKEND=b200)
 """
 import ctypes as C
 import glob
+import gzip
 import io
 import os
 import struct
 import tarfile
 import time
+import urllib.request
 
 import numpy as np
 
@@ -183,3 +194,137 @@ def create_compressed_tarball(package_build, ctx=None):
     home = os.environ["HOME"]
     tarball_path = f"{home}/.lambdipy/build/{package_build.git_tag()}.tar.gz"
     return gzip_tarball(glob.glob(f"{package_build.build_directory()}/*"), tarball_path, ctx)
+
+
+# ---- reading ------------------------------------------------------------------------------------------------------
+FTEXT, FHCRC, FEXTRA, FNAME, FCOMMENT = 1, 2, 4, 8, 16
+
+
+class InflateDataError(gzip.BadGzipFile):
+    """The DEFLATE body of a member is invalid or truncated (LB2_E_DATA)."""
+
+
+def gzip_members(buf):
+    """Yields the offset of each gzip member's DEFLATE body in `buf`, and expects the generator to be sent the
+    number of body bytes the member used; checks framing as gzip.GzipFile does (magic, CM = 8, the FEXTRA / FNAME /
+    FCOMMENT / FHCRC fields, zero padding between and after members) and refuses reserved flag bits."""
+    n, pos = len(buf), 0
+    while True:
+        while pos < n and buf[pos] == 0:
+            pos += 1
+        if pos >= n:
+            return
+        if n - pos < 2 or bytes(buf[pos:pos + 2]) != b"\037\213":
+            raise gzip.BadGzipFile("Not a gzipped file (%r)" % bytes(buf[pos:pos + 2]))
+        if n - pos < 10:
+            raise EOFError("Compressed file ended before the end-of-stream marker was reached")
+        method, flag = buf[pos + 2], buf[pos + 3]
+        if method != 8:
+            raise gzip.BadGzipFile("Unknown compression method")
+        if flag & 0xE0:
+            raise gzip.BadGzipFile("Reserved gzip header flags set (0x%02x)" % flag)
+        p = pos + 10
+        if flag & FEXTRA:
+            if n - p < 2:
+                raise EOFError("Compressed file ended before the end-of-stream marker was reached")
+            p += 2 + (buf[p] | buf[p + 1] << 8)
+        for f in (FNAME, FCOMMENT):
+            if flag & f:
+                z = bytes(buf[p:]).find(b"\0") if p < n else -1
+                if z < 0:
+                    raise EOFError("Compressed file ended before the end-of-stream marker was reached")
+                p += z + 1
+        if flag & FHCRC:
+            p += 2
+        if p > n:
+            raise EOFError("Compressed file ended before the end-of-stream marker was reached")
+        used = yield p
+        pos = p + used + 8
+        if pos > n:
+            raise EOFError("Compressed file ended before the end-of-stream marker was reached")
+
+
+def gunzip(path, ctx=None):
+    """The decompressed contents of the gzip file at `path` (all members), decoded on the GPU.
+
+    Raises gzip.BadGzipFile for bad framing or a CRC / ISIZE mismatch, InflateDataError (a BadGzipFile) for an
+    invalid DEFLATE body, EOFError for a truncated file, and NativeError with code LB2_E_CAPACITY when a member does
+    not fit in device memory.  ctx=None: the context of _default_context()."""
+    own = False
+    if ctx is None:
+        ctx, own = _default_context()
+    lib, h_in, d, outs = ctx.lib, None, None, []
+    try:
+        size = os.path.getsize(path)
+        h_in = ctx.pinned_alloc(max(size, 1))
+        buf = (C.c_uint8 * size).from_address(h_in) if size else bytearray()
+        with open(path, "rb") as f:
+            if size and f.readinto(memoryview(buf).cast("B")) != size:
+                raise EOFError("%s changed while it was read" % path)
+        h = C.c_void_p()
+        ctx.check(lib.lb2_inflate_create(ctx.h, 0, C.byref(h)))
+        d = h
+        members = gzip_members(memoryview(buf).cast("B") if size else buf)
+        body = next(members, None)
+        while body is not None:
+            out_n, st = C.c_uint64(), N.InflateStats()
+            rc = lib.lb2_inflate_run(d, h_in + body, size - body, C.byref(out_n), C.byref(st))
+            if rc == N.LB2_E_DATA:
+                raise InflateDataError("%s: %s" % (path, (lib.lb2_last_error(ctx.h) or b"").decode()))
+            ctx.check(rc)
+            crc, isize = st.crc32, out_n.value
+            out = ctx.pinned_alloc(max(isize, 1))
+            outs.append((out, isize))
+            ctx.check(lib.lb2_inflate_read(d, out, isize))
+            t = body + st.in_bytes
+            if size - t < 8:
+                raise EOFError("Compressed file ended before the end-of-stream marker was reached")
+            want_crc, want_isize = struct.unpack_from("<II", buf, t)
+            if want_crc != crc:
+                raise gzip.BadGzipFile("CRC check failed")
+            if want_isize != isize & 0xFFFFFFFF:
+                raise gzip.BadGzipFile("Incorrect length of data produced")
+            try:
+                body = members.send(st.in_bytes)
+            except StopIteration:
+                body = None
+        # the one host copy: pinned staging -> the returned bytes
+        return b"".join(memoryview((C.c_uint8 * n).from_address(p)).cast("B") for p, n in outs if n)
+    finally:
+        if d is not None:
+            lib.lb2_inflate_destroy(d)
+        for p, _ in outs:
+            ctx.pinned_free(p)
+        if h_in is not None:
+            ctx.pinned_free(h_in)
+        if own:
+            ctx.close()
+
+
+def extract_tarball(tarball_path, directory, ctx=None):
+    """tarfile.open(tarball_path, "r:gz").extractall(directory), with the gzip layer decoded on the GPU: the
+    standard library still parses the tar stream and writes the files, with the running Python's defaults."""
+    with tarfile.open(fileobj=io.BytesIO(gunzip(tarball_path, ctx)), mode="r:") as tar:
+        tar.extractall(directory)
+
+
+def prepare_tarfile(url, download_filename, package_directory):
+    """Mirror of the reference's prepare_tarfile (lambdipy/project_build.py:98-102): download, then extract.  A file
+    the GPU reader refuses (bad framing or data, a trailer mismatch, too large for the device) is handed to the
+    reference's own two lines, which raise what the reference raises and leave what it leaves."""
+    urllib.request.urlretrieve(url, download_filename)
+    try:
+        extract_tarball(download_filename, package_directory)
+    except (gzip.BadGzipFile, EOFError) as e:
+        _reference_extract(download_filename, package_directory, e)
+    except N.NativeError as e:
+        if e.code != N.LB2_E_CAPACITY:
+            raise
+        _reference_extract(download_filename, package_directory, e)
+
+
+def _reference_extract(download_filename, package_directory, why):
+    print("lambdipy_b200: %s: %s; extracting with tarfile" % (download_filename, why))
+    tar = tarfile.open(download_filename, "r:gz")
+    tar.extractall(package_directory)
+    tar.close()
