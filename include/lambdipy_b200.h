@@ -244,6 +244,49 @@ int lb2_gzip_finish(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n,
                     lb2_gzip_stats *stats);
 void lb2_gzip_destroy(lb2_gzip *g);
 
+/* ---- zip writer: one raw DEFLATE stream + CRC-32 per file, many files per piece ------------------ */
+/* What `shutil.make_archive(base, "zip", "./build")` spends its time on when a Lambda bundle is zipped: every
+ * zip member is its own raw DEFLATE stream.  The caller writes the zip container (headers, central directory);
+ * the library produces each member's body and CRC-32.
+ *
+ * A piece holds n_segs segments, one per file (or part of a file): segment i is h_in[seg_off[i] ..
+ * + seg_len[i]), seg_off[i] a multiple of 16, in increasing order without overlap.  Each segment is deflated
+ * like a gzip piece (64 KB chunks, sync-flushed, dynamic / fixed / stored per chunk), but no chunk crosses a
+ * segment and no match reaches into another file; a file that ends in the piece is closed with the 2-byte final
+ * block 03 00, so an empty file's body is exactly 03 00 (as zlib's).  Each member costs at most 5 + 2 bytes of
+ * framing per 64 KB chunk, plus 2 for its final block, over its stored size.
+ *
+ * A file larger than a piece continues into the next one: submit its first part as the LAST segment with
+ * LB2_ZIP_MORE, and its rest as segment 0 (seg_off[0] = 0) of the next piece with LB2_ZIP_CONTINUES; the
+ * library keeps the file's last 32 KB on the device as history and its running CRC-32.  Chunks start at
+ * multiples of 64 KB of each segment, so cut a file at a multiple of 64 KB of its bytes: it is then deflated in
+ * the chunks (and within the bound) of the whole file; a cut elsewhere costs one more chunk per piece boundary.
+ *
+ * Up to TWO pieces may be in flight, as with lb2_gzip_*.  lb2_zip_collect waits for the OLDEST piece, copies
+ * its DEFLATE bytes (all segments back to back) to h_out and fills segs[0 .. n_segs) of that piece: where each
+ * segment's bytes are in h_out, the CRC-32 of its file from the file's first byte (earlier pieces included),
+ * and whether the file ended.  stats (may be NULL) receives the totals so far; its crc32 is the running CRC-32
+ * of the file left open (0 if none).  The same pieces always give the same bytes.  Destroy the writer before its
+ * context. */
+typedef struct lb2_zip lb2_zip;
+typedef struct lb2_zip_segment {
+  uint64_t out_off, out_len;   /* the segment's DEFLATE bytes in the collected output                       */
+  uint32_t crc32;              /* CRC-32 of the file so far                                                 */
+  uint32_t ended;              /* 1: the file ended in this piece; its bytes end with the final block       */
+} lb2_zip_segment;
+#define LB2_ZIP_CONTINUES 1u   /* segment 0 continues the file the previous piece left open                 */
+#define LB2_ZIP_MORE      2u   /* the last segment's file continues in the next piece                       */
+/* worst-case DEFLATE bytes of one piece of n bytes (padding included) in n_segs segments (out_cap of lb2_zip_collect) */
+#define LB2_ZIP_BOUND(n, n_segs) (LB2_GZIP_BOUND(n) + 17 * (uint64_t)(n_segs))
+int lb2_zip_create(lb2_ctx *ctx, uint32_t flags /* 0 */, lb2_zip **z);
+/* LB2_E_STATE: two pieces in flight, LB2_ZIP_CONTINUES without an open file, or an open file not continued */
+int lb2_zip_submit(lb2_zip *z, const void *h_in, uint64_t n, const uint64_t *seg_off, const uint64_t *seg_len,
+                   uint32_t n_segs, uint32_t flags);
+/* LB2_E_CAPACITY when out_cap is too small: *out_n says how much is needed, the piece stays in flight */
+int lb2_zip_collect(lb2_zip *z, void *h_out, uint64_t out_cap, uint64_t *out_n, lb2_zip_segment *segs,
+                    lb2_gzip_stats *stats);
+void lb2_zip_destroy(lb2_zip *z);
+
 /* ---- gzip reader: raw DEFLATE (RFC 1951) decoded on the GPU ----------------------------------- */
 /* What `tarfile.open(path, "r:gz")` spends its time on in prepare_tarfile (lambdipy/project_build.py:98-102 of the
  * reference).  The caller parses the gzip header and trailer; the library decodes the DEFLATE body in between.

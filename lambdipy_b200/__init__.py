@@ -9,6 +9,8 @@ Public surface:
     tarball.create_compressed_tarball           mirror of PackageBuild.create_compressed_tarball
     gunzip(path)                                decompressed bytes of a gzip file, DEFLATE decoded on the GPU
     tarball.prepare_tarfile                     mirror of the reference's prepare_tarfile
+    zip_tree(root_dir, zip_path)                the Lambda deployment zip of a tree (shutil.make_archive's
+                                                archive), every member's DEFLATE body compressed on the GPU
     patch.apply()                               monkey-patch an installed lambdipy in place
 The byte work is done by liblambdipy_b200.so (CUDA, C ABI in include/lambdipy_b200.h).
 """
@@ -22,4 +24,7 @@ def __getattr__(name):
     if name in ("gzip_tarball", "gunzip"):
         from . import tarball
         return getattr(tarball, name)
+    if name == "zip_tree":
+        from . import zipfile_gpu
+        return zipfile_gpu.zip_tree
     raise AttributeError(name)

@@ -26,7 +26,9 @@ EXPORTS = [
     "lb2_strip_device_chunked", "lb2_tree_prepare", "lb2_strip_tree_ex", "lb2_tree_cleanup",
     "lb2_gzip_create", "lb2_gzip_submit", "lb2_gzip_collect", "lb2_gzip_finish", "lb2_gzip_destroy",
     "lb2_inflate_create", "lb2_inflate_run", "lb2_inflate_read", "lb2_inflate_destroy",
+    "lb2_zip_create", "lb2_zip_submit", "lb2_zip_collect", "lb2_zip_destroy",
 ]
+ZIP_CONTINUES, ZIP_MORE = 1, 2
 
 
 def gzip_bound(n):
@@ -72,6 +74,15 @@ class GzipStats(C.Structure):
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+def zip_bound(n, n_segs):
+    """worst-case DEFLATE bytes of one zip piece of n bytes in n_segs segments (LB2_ZIP_BOUND)"""
+    return gzip_bound(n) + 17 * n_segs
+
+
+class ZipSegment(C.Structure):
+    _fields_ = [("out_off", C.c_uint64), ("out_len", C.c_uint64), ("crc32", C.c_uint32), ("ended", C.c_uint32)]
 
 
 class InflateStats(C.Structure):
@@ -178,6 +189,14 @@ def load():
     lib.lb2_inflate_read.restype = C.c_int
     lib.lb2_inflate_destroy.argtypes = [vp]
     lib.lb2_inflate_destroy.restype = None
+    lib.lb2_zip_create.argtypes = [vp, C.c_uint32, C.POINTER(vp)]
+    lib.lb2_zip_create.restype = C.c_int
+    lib.lb2_zip_submit.argtypes = [vp, vp, C.c_uint64, u64p, u64p, C.c_uint32, C.c_uint32]
+    lib.lb2_zip_submit.restype = C.c_int
+    lib.lb2_zip_collect.argtypes = [vp, vp, C.c_uint64, u64p, C.POINTER(ZipSegment), C.POINTER(GzipStats)]
+    lib.lb2_zip_collect.restype = C.c_int
+    lib.lb2_zip_destroy.argtypes = [vp]
+    lib.lb2_zip_destroy.restype = None
     _lib = lib
     return lib
 

@@ -1,6 +1,6 @@
 // api.cu -- C ABI (include/lambdipy_b200.h) over the plan / scan / compaction kernels: the context, the batch core
 // that every strip path queues its batches through, the entry points on device-resident arenas, the corpus helpers
-// and the host side of the gzip writer and reader.  The host-buffer pipelines of lb2_strip_host are in
+// and the host side of the gzip and zip writers and of the gzip reader.  The host-buffer pipelines of lb2_strip_host are in
 // strip_host.cu, the tree walker and its streaming engine in strip_tree.cu.
 #include "lb2_host.cuh"
 
@@ -473,156 +473,198 @@ int lb2_corpus_scatter(lb2_ctx *ctx, void *d_arena, const void *h_data, uint64_t
 
 }  // extern "C"
 
-// ---------------------------------------------------------------------------- gzip writer
-// Device buffers of one piece in flight.  d_in holds GZ_HIST bytes of history in front of the piece: the tail of
-// the stream so far, copied there from lb2_gzip::d_hist, so every chunk can look back 32 KB across piece boundaries.
+// ---------------------------------------------------------------------------- gzip and zip writers
+// Device buffers of one piece in flight.  d_in holds GZ_HIST bytes of history in front of the piece: the tail of the
+// stream (gzip) or of the file (zip) that the previous piece left open, copied there from GzWriter::d_hist, so the
+// first segment's chunks can look back 32 KB across piece boundaries.  The chunk and segment tables are built on the
+// host in h_tab and uploaded with the piece.
 struct GzSlot {
   uint8_t *d_in = nullptr, *d_chunk_out = nullptr, *d_out = nullptr;
   uint32_t *d_tok = nullptr, *d_meta = nullptr;  // meta: size | mode | crc, n_chunks each
   uint64_t *d_off = nullptr;
+  uint8_t *d_tab = nullptr, *h_tab = nullptr;    // GzChunk[n_chunks] then GzSeg[n_segs]
+  GzSegResult *d_seg = nullptr, *h_seg = nullptr;  // per-segment results (lb2_zip_segment layout)
   GzResult *d_res = nullptr, *h_res = nullptr;
-  uint32_t cap_chunks = 0;
+  uint64_t cap_bytes = 0, cap_tab = 0;
+  uint32_t cap_chunks = 0, cap_segs = 0;
   cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // upload | deflate | crc | compact |
   cudaEvent_t done = nullptr;
-  uint64_t n = 0;
+  uint32_t n_segs = 0;
 };
 
-struct lb2_gzip {
+struct GzWriter {
   lb2_ctx *ctx = nullptr;
   cudaStream_t stream = nullptr;
-  uint8_t *d_hist = nullptr;   // last <= GZ_HIST bytes of the stream
-  uint32_t *d_crc = nullptr;   // running CRC-32, advanced by each piece's scan kernel
+  uint8_t *d_hist = nullptr;   // last <= GZ_HIST bytes of the open stream / file
+  uint32_t *d_crc = nullptr;   // running CRC-32 of the open stream / file, advanced by each piece's scan kernel
   uint64_t hist_len = 0;
+  bool open = false;           // the last piece submitted left a file open (zip)
   GzSlot slot[2];
   int head = 0, count = 0;     // pieces in flight, collected in submission order
   bool finished = false;
   lb2_gzip_stats st{};
 };
+struct lb2_gzip : GzWriter {};
+struct lb2_zip : GzWriter {};
 
 static void gz_slot_free(GzSlot &s) {
   cudaFree(s.d_in); cudaFree(s.d_chunk_out); cudaFree(s.d_out); cudaFree(s.d_tok); cudaFree(s.d_meta); cudaFree(s.d_off);
-  cudaFree(s.d_res);
+  cudaFree(s.d_tab); cudaFree(s.d_seg); cudaFree(s.d_res);
+  if (s.h_tab) cudaFreeHost(s.h_tab);
+  if (s.h_seg) cudaFreeHost(s.h_seg);
   if (s.h_res) cudaFreeHost(s.h_res);
   for (auto &e : s.ev) if (e) cudaEventDestroy(e);
   if (s.done) cudaEventDestroy(s.done);
   s = GzSlot();
 }
 
-static int gz_slot_reserve(lb2_ctx *ctx, GzSlot &s, uint32_t n_chunks) {
+static int gz_slot_reserve(lb2_ctx *ctx, GzSlot &s, uint64_t n, uint32_t n_chunks, uint32_t n_segs) {
   if (!s.d_res) {
     CK(cudaMalloc(&s.d_res, sizeof(GzResult)));
     CK(cudaHostAlloc(&s.h_res, sizeof(GzResult), cudaHostAllocDefault));
     for (auto &e : s.ev) CK(cudaEventCreate(&e));
     CK(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
   }
-  if (n_chunks <= s.cap_chunks) return LB2_OK;
-  cudaFree(s.d_in); cudaFree(s.d_chunk_out); cudaFree(s.d_out); cudaFree(s.d_tok); cudaFree(s.d_meta); cudaFree(s.d_off);
-  s.d_in = s.d_chunk_out = s.d_out = nullptr; s.d_tok = s.d_meta = nullptr; s.d_off = nullptr;
-  s.cap_chunks = 0;
-  const uint64_t n = n_chunks;
-  CK(cudaMalloc(&s.d_in, GZ_HIST + n * GZ_CHUNK + 16));
-  CK(cudaMalloc(&s.d_chunk_out, n * GZ_CHUNK_OUT_CAP));
-  CK(cudaMalloc(&s.d_out, n * (GZ_CHUNK + 15) + 16));
-  CK(cudaMalloc(&s.d_tok, n * GZ_CHUNK * sizeof(uint32_t)));
-  CK(cudaMalloc(&s.d_meta, 3 * n * sizeof(uint32_t)));
-  CK(cudaMalloc(&s.d_off, n * sizeof(uint64_t)));
-  s.cap_chunks = n_chunks;
+  if (n > s.cap_bytes || n_chunks > s.cap_chunks) {
+    const uint64_t b = std::max(n, s.cap_bytes), c = std::max(n_chunks, s.cap_chunks);
+    cudaFree(s.d_in); cudaFree(s.d_chunk_out); cudaFree(s.d_out); cudaFree(s.d_tok); cudaFree(s.d_meta); cudaFree(s.d_off);
+    s.d_in = s.d_chunk_out = s.d_out = nullptr; s.d_tok = s.d_meta = nullptr; s.d_off = nullptr;
+    s.cap_bytes = 0; s.cap_chunks = 0;
+    CK(cudaMalloc(&s.d_in, GZ_HIST + b + 16));
+    CK(cudaMalloc(&s.d_chunk_out, b + GZ_OUT_PAD * c + 64));
+    CK(cudaMalloc(&s.d_out, b + 17 * c + 16));  // <= 15 bytes of framing per chunk, 2 per segment (segments <= chunks)
+    CK(cudaMalloc(&s.d_tok, b * sizeof(uint32_t) + 16));
+    CK(cudaMalloc(&s.d_meta, 3 * c * sizeof(uint32_t)));
+    CK(cudaMalloc(&s.d_off, c * sizeof(uint64_t)));
+    s.cap_bytes = b; s.cap_chunks = (uint32_t)c;
+  }
+  const uint64_t tab = (uint64_t)n_chunks * sizeof(GzChunk) + (uint64_t)n_segs * sizeof(GzSeg);
+  if (tab > s.cap_tab) {
+    const uint64_t t = std::max(tab, 2 * s.cap_tab);
+    cudaFree(s.d_tab);
+    if (s.h_tab) cudaFreeHost(s.h_tab);
+    s.d_tab = s.h_tab = nullptr;
+    s.cap_tab = 0;
+    CK(cudaMalloc(&s.d_tab, t));
+    CK(cudaHostAlloc(&s.h_tab, t, cudaHostAllocDefault));
+    s.cap_tab = t;
+  }
+  if (n_segs > s.cap_segs) {
+    cudaFree(s.d_seg);
+    if (s.h_seg) cudaFreeHost(s.h_seg);
+    s.d_seg = s.h_seg = nullptr;
+    s.cap_segs = 0;
+    CK(cudaMalloc(&s.d_seg, n_segs * sizeof(GzSegResult)));
+    CK(cudaHostAlloc(&s.h_seg, n_segs * sizeof(GzSegResult), cudaHostAllocDefault));
+    s.cap_segs = n_segs;
+  }
   return LB2_OK;
 }
 
-extern "C" {
-
-int lb2_gzip_create(lb2_ctx *ctx, uint32_t flags, lb2_gzip **out) {
-  if (!ctx || !out) { if (ctx) ctx->err = "NULL argument"; return LB2_E_ARG; }
-  *out = nullptr;
-  if (flags) { ctx->err = "lb2_gzip_create: no flags are defined"; return LB2_E_ARG; }
-  CK(cudaSetDevice(ctx->device));
-  lb2_gzip *g = new lb2_gzip();
+static int gz_create(lb2_ctx *ctx, GzWriter *g, const char *what) {
   g->ctx = ctx;
+  CK(cudaSetDevice(ctx->device));
   cudaError_t e;
   if ((e = cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking)) != cudaSuccess ||
       (e = cudaMalloc(&g->d_hist, GZ_HIST)) != cudaSuccess || (e = cudaMalloc(&g->d_crc, sizeof(uint32_t))) != cudaSuccess ||
       (e = cudaMemsetAsync(g->d_crc, 0, sizeof(uint32_t), g->stream)) != cudaSuccess) {
-    ctx->err = std::string("lb2_gzip_create: ") + cudaGetErrorString(e);
-    lb2_gzip_destroy(g);
+    ctx->err = std::string(what) + ": " + cudaGetErrorString(e);
     return LB2_E_CUDA;
   }
-  *out = g;
   return LB2_OK;
 }
 
-void lb2_gzip_destroy(lb2_gzip *g) {
-  if (!g) return;
+static void gz_destroy(GzWriter *g) {
   cudaSetDevice(g->ctx->device);
   if (g->stream) cudaStreamSynchronize(g->stream);
   for (auto &s : g->slot) gz_slot_free(s);
   cudaFree(g->d_hist);
   cudaFree(g->d_crc);
   if (g->stream) cudaStreamDestroy(g->stream);
-  delete g;
 }
 
-int lb2_gzip_submit(lb2_gzip *g, const void *h_in, uint64_t n) {
-  if (!g) return LB2_E_ARG;
+// Enqueue one piece of n bytes at h_in holding n_segs segments [seg_off[i], seg_off[i] + seg_len[i]) (validated by
+// the caller).  cont: segment 0 continues the open stream / file; ends: segment i's file ends in this piece.
+static int gz_submit(GzWriter *g, const void *h_in, uint64_t n, const uint64_t *seg_off, const uint64_t *seg_len,
+                     uint32_t n_segs, bool cont, bool last_ends) {
   lb2_ctx *ctx = g->ctx;
-  if (!h_in && n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
-  if (g->finished) { ctx->err = "lb2_gzip_submit after lb2_gzip_finish"; return LB2_E_STATE; }
-  if (g->count >= 2) { ctx->err = "two pieces already in flight: collect one with lb2_gzip_collect first"; return LB2_E_STATE; }
-  if (n > (uint64_t)UINT32_MAX * GZ_CHUNK / 2) { ctx->err = "piece too large"; return LB2_E_ARG; }
   CK(cudaSetDevice(ctx->device));
   GzSlot &s = g->slot[(g->head + g->count) & 1];
-  s.n = n;
-  if (n) {
-    const uint32_t n_chunks = (uint32_t)((n + GZ_CHUNK - 1) / GZ_CHUNK);
-    int rc = gz_slot_reserve(ctx, s, n_chunks);
-    if (rc) return rc;
-    cudaStream_t st = g->stream;
-    GzPieceArgs a;
-    a.in = s.d_in + GZ_HIST; a.n = n; a.hist = (uint32_t)g->hist_len; a.n_chunks = n_chunks;
-    a.tokens = s.d_tok; a.chunk_out = s.d_chunk_out;
-    a.chunk_size = s.d_meta; a.chunk_mode = s.d_meta + n_chunks; a.chunk_crc = s.d_meta + 2 * n_chunks;
-    a.chunk_off = s.d_off; a.out = s.d_out; a.crc_state = g->d_crc; a.res = s.d_res;
-    CK(cudaEventRecord(s.ev[0], st));
-    if (g->hist_len)
-      CK(cudaMemcpyAsync(s.d_in + GZ_HIST - g->hist_len, g->d_hist, g->hist_len, cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(s.d_in + GZ_HIST, h_in, n, cudaMemcpyHostToDevice, st));
-    CK(cudaEventRecord(s.ev[1], st));
-    launch_deflate(a, st);
-    CK(cudaEventRecord(s.ev[2], st));
-    launch_crc32(a, st);
-    CK(cudaEventRecord(s.ev[3], st));
-    launch_gzip_compact(a, st);
-    CK(cudaEventRecord(s.ev[4], st));
-    CK(cudaMemcpyAsync(s.h_res, s.d_res, sizeof(GzResult), cudaMemcpyDeviceToHost, st));
-    CK(cudaEventRecord(s.done, st));
-    // history of the next piece: the stream's last <= 32 KB, which end with this piece
-    const uint64_t keep = std::min<uint64_t>(GZ_HIST, g->hist_len + n);
-    CK(cudaMemcpyAsync(g->d_hist, s.d_in + GZ_HIST + n - keep, keep, cudaMemcpyDeviceToDevice, st));
-    CK(cudaGetLastError());
-    g->hist_len = keep;
-    g->st.n_chunks += n_chunks;
+  uint64_t n_chunks = 0;
+  for (uint32_t i = 0; i < n_segs; i++) n_chunks += seg_len[i] ? (seg_len[i] + GZ_CHUNK - 1) / GZ_CHUNK : 1;
+  if (n_chunks > UINT32_MAX / 2) { ctx->err = "piece too large"; return LB2_E_ARG; }
+  int rc = gz_slot_reserve(ctx, s, n, (uint32_t)n_chunks, n_segs);
+  if (rc) return rc;
+  GzChunk *chunks = reinterpret_cast<GzChunk *>(s.h_tab);
+  GzSeg *segs = reinterpret_cast<GzSeg *>(s.h_tab + n_chunks * sizeof(GzChunk));
+  uint32_t c = 0, n_data = 0;
+  for (uint32_t i = 0; i < n_segs; i++) {
+    const bool ends = i + 1 < n_segs || last_ends;
+    const uint64_t before = i == 0 && cont ? g->hist_len : 0;  // bytes of the segment's file in front of it
+    segs[i] = GzSeg{seg_off[i], seg_len[i], c, (i == 0 && cont ? GZ_SEG_CONTINUES : 0u) | (ends ? GZ_SEG_ENDS : 0u)};
+    uint64_t p = 0;
+    do {
+      const uint32_t len = (uint32_t)std::min<uint64_t>(GZ_CHUNK, seg_len[i] - p);
+      const uint32_t hist = (uint32_t)std::min<uint64_t>(GZ_HIST, before + p);
+      chunks[c++] = GzChunk{seg_off[i] + p, len, hist, i, ends && p + len == seg_len[i]};
+      n_data += len != 0;
+      p += len;
+    } while (p < seg_len[i]);
   }
+  cudaStream_t st = g->stream;
+  GzPieceArgs a;
+  a.in = s.d_in + GZ_HIST; a.n = n; a.n_chunks = c; a.n_segs = n_segs;
+  a.chunks = reinterpret_cast<const GzChunk *>(s.d_tab);
+  a.segs = reinterpret_cast<const GzSeg *>(s.d_tab + n_chunks * sizeof(GzChunk));
+  a.tokens = s.d_tok; a.chunk_out = s.d_chunk_out;
+  a.chunk_size = s.d_meta; a.chunk_mode = s.d_meta + c; a.chunk_crc = s.d_meta + 2 * c;
+  a.chunk_off = s.d_off; a.out = s.d_out; a.crc_state = g->d_crc; a.seg_res = s.d_seg; a.res = s.d_res;
+  CK(cudaEventRecord(s.ev[0], st));
+  if (cont && g->hist_len)
+    CK(cudaMemcpyAsync(s.d_in + GZ_HIST - g->hist_len, g->d_hist, g->hist_len, cudaMemcpyDeviceToDevice, st));
+  if (n) CK(cudaMemcpyAsync(s.d_in + GZ_HIST, h_in, n, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(s.d_tab, s.h_tab, n_chunks * sizeof(GzChunk) + n_segs * sizeof(GzSeg), cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(s.ev[1], st));
+  launch_deflate(a, st);
+  CK(cudaEventRecord(s.ev[2], st));
+  launch_crc32(a, st);
+  CK(cudaEventRecord(s.ev[3], st));
+  launch_gzip_compact(a, st);
+  CK(cudaEventRecord(s.ev[4], st));
+  CK(cudaMemcpyAsync(s.h_res, s.d_res, sizeof(GzResult), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(s.h_seg, s.d_seg, n_segs * sizeof(GzSegResult), cudaMemcpyDeviceToHost, st));
+  CK(cudaEventRecord(s.done, st));
+  // history of the next piece: the last <= 32 KB of the file or stream left open, which end with this piece
+  uint64_t keep = 0;
+  if (!last_ends) {
+    const GzSeg &l = segs[n_segs - 1];
+    keep = std::min<uint64_t>(GZ_HIST, l.len + (n_segs == 1 && cont ? g->hist_len : 0));
+    if (keep) CK(cudaMemcpyAsync(g->d_hist, s.d_in + GZ_HIST + l.start + l.len - keep, keep, cudaMemcpyDeviceToDevice, st));
+  }
+  CK(cudaGetLastError());
+  g->hist_len = keep;
+  g->open = !last_ends;
+  g->st.n_chunks += n_data;
   g->st.in_bytes += n;
+  s.n_segs = n_segs;
   g->count++;
   return LB2_OK;
 }
 
-int lb2_gzip_collect(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n) {
-  if (!g) return LB2_E_ARG;
+// Wait for the oldest piece and copy its bytes (and, if segs, its per-segment results) out.
+static int gz_collect(GzWriter *g, void *h_out, uint64_t out_cap, uint64_t *out_n, GzSegResult *segs) {
   lb2_ctx *ctx = g->ctx;
-  if (!out_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
-  if (!g->count) { ctx->err = "no piece in flight"; return LB2_E_STATE; }
   CK(cudaSetDevice(ctx->device));
   GzSlot &s = g->slot[g->head];
   uint64_t total = 0;
-  if (s.n) {
+  if (s.n_segs) {
     CK(cudaEventSynchronize(s.done));
     total = s.h_res->out_bytes;
     *out_n = total;
     if (total > out_cap) { ctx->err = "output buffer too small for this piece (*out_n bytes needed)"; return LB2_E_CAPACITY; }
     if (!h_out) { ctx->err = "NULL argument"; return LB2_E_ARG; }
     const double t0 = now_s();
-    CK(cudaMemcpy(h_out, s.d_out, total, cudaMemcpyDeviceToHost));
+    if (total) CK(cudaMemcpy(h_out, s.d_out, total, cudaMemcpyDeviceToHost));
     g->st.d2h_ms += (float)((now_s() - t0) * 1e3);
     float ms = 0;
     CK(cudaEventElapsedTime(&ms, s.ev[0], s.ev[1])); g->st.h2d_ms += ms;
@@ -633,11 +675,57 @@ int lb2_gzip_collect(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n
     g->st.n_stored_chunks += s.h_res->n_stored;
     g->st.n_fixed_chunks += s.h_res->n_fixed;
     g->st.out_bytes += total;
+    if (segs) std::copy(s.h_seg, s.h_seg + s.n_segs, segs);
   }
   *out_n = total;
+  s.n_segs = 0;
   g->head ^= 1;
   g->count--;
   return LB2_OK;
+}
+
+extern "C" {
+
+int lb2_gzip_create(lb2_ctx *ctx, uint32_t flags, lb2_gzip **out) {
+  if (!ctx || !out) { if (ctx) ctx->err = "NULL argument"; return LB2_E_ARG; }
+  *out = nullptr;
+  if (flags) { ctx->err = "lb2_gzip_create: no flags are defined"; return LB2_E_ARG; }
+  lb2_gzip *g = new lb2_gzip();
+  const int rc = gz_create(ctx, g, "lb2_gzip_create");
+  if (rc) { lb2_gzip_destroy(g); return rc; }
+  *out = g;
+  return LB2_OK;
+}
+
+void lb2_gzip_destroy(lb2_gzip *g) {
+  if (!g) return;
+  gz_destroy(g);
+  delete g;
+}
+
+int lb2_gzip_submit(lb2_gzip *g, const void *h_in, uint64_t n) {
+  if (!g) return LB2_E_ARG;
+  lb2_ctx *ctx = g->ctx;
+  if (!h_in && n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if (g->finished) { ctx->err = "lb2_gzip_submit after lb2_gzip_finish"; return LB2_E_STATE; }
+  if (g->count >= 2) { ctx->err = "two pieces already in flight: collect one with lb2_gzip_collect first"; return LB2_E_STATE; }
+  if (n > (uint64_t)UINT32_MAX * GZ_CHUNK / 2) { ctx->err = "piece too large"; return LB2_E_ARG; }
+  if (!n) {  // nothing to deflate: collect returns 0 bytes
+    g->slot[(g->head + g->count) & 1].n_segs = 0;
+    g->count++;
+    return LB2_OK;
+  }
+  // the piece is one segment of the stream, which continues from the previous piece and stays open
+  const uint64_t off = 0;
+  return gz_submit(g, h_in, n, &off, &n, 1, true, false);
+}
+
+int lb2_gzip_collect(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n) {
+  if (!g) return LB2_E_ARG;
+  lb2_ctx *ctx = g->ctx;
+  if (!out_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if (!g->count) { ctx->err = "no piece in flight"; return LB2_E_STATE; }
+  return gz_collect(g, h_out, out_cap, out_n, nullptr);
 }
 
 int lb2_gzip_finish(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n, uint32_t *crc32, uint64_t *isize,
@@ -658,6 +746,59 @@ int lb2_gzip_finish(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n,
   if (isize) *isize = g->st.in_bytes;
   if (stats) *stats = g->st;
   return LB2_OK;
+}
+
+static_assert(sizeof(GzSegResult) == sizeof(lb2_zip_segment), "the scan kernel writes lb2_zip_segment records");
+
+int lb2_zip_create(lb2_ctx *ctx, uint32_t flags, lb2_zip **out) {
+  if (!ctx || !out) { if (ctx) ctx->err = "NULL argument"; return LB2_E_ARG; }
+  *out = nullptr;
+  if (flags) { ctx->err = "lb2_zip_create: no flags are defined"; return LB2_E_ARG; }
+  lb2_zip *z = new lb2_zip();
+  const int rc = gz_create(ctx, z, "lb2_zip_create");
+  if (rc) { lb2_zip_destroy(z); return rc; }
+  *out = z;
+  return LB2_OK;
+}
+
+void lb2_zip_destroy(lb2_zip *z) {
+  if (!z) return;
+  gz_destroy(z);
+  delete z;
+}
+
+int lb2_zip_submit(lb2_zip *z, const void *h_in, uint64_t n, const uint64_t *seg_off, const uint64_t *seg_len, uint32_t n_segs,
+                   uint32_t flags) {
+  if (!z) return LB2_E_ARG;
+  lb2_ctx *ctx = z->ctx;
+  if ((!h_in && n) || !seg_off || !seg_len) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if (flags & ~(LB2_ZIP_CONTINUES | LB2_ZIP_MORE)) { ctx->err = "lb2_zip_submit: unknown flags"; return LB2_E_ARG; }
+  if (!n_segs) { ctx->err = "a piece holds at least one segment"; return LB2_E_ARG; }
+  if (n > (uint64_t)UINT32_MAX * GZ_CHUNK / 2) { ctx->err = "piece too large"; return LB2_E_ARG; }
+  if (z->count >= 2) { ctx->err = "two pieces already in flight: collect one with lb2_zip_collect first"; return LB2_E_STATE; }
+  const bool cont = flags & LB2_ZIP_CONTINUES;
+  if (cont && !z->open) { ctx->err = "LB2_ZIP_CONTINUES, but the previous piece left no file open"; return LB2_E_STATE; }
+  if (!cont && z->open) { ctx->err = "the previous piece's last file is still open: continue it with LB2_ZIP_CONTINUES"; return LB2_E_STATE; }
+  if (cont && seg_off[0]) { ctx->err = "a continued file starts the piece: seg_off[0] must be 0"; return LB2_E_ARG; }
+  uint64_t end = 0;
+  for (uint32_t i = 0; i < n_segs; i++) {
+    if ((seg_off[i] & 15) || seg_off[i] < end || seg_off[i] > n || seg_len[i] > n - seg_off[i]) {
+      ctx->err = "segment " + std::to_string(i) + " is unaligned, overlaps the one before it or ends past the piece";
+      return LB2_E_ARG;
+    }
+    end = seg_off[i] + seg_len[i];
+  }
+  return gz_submit(z, h_in, n, seg_off, seg_len, n_segs, cont, !(flags & LB2_ZIP_MORE));
+}
+
+int lb2_zip_collect(lb2_zip *z, void *h_out, uint64_t out_cap, uint64_t *out_n, lb2_zip_segment *segs, lb2_gzip_stats *stats) {
+  if (!z) return LB2_E_ARG;
+  lb2_ctx *ctx = z->ctx;
+  if (!out_n || !segs) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if (!z->count) { ctx->err = "no piece in flight"; return LB2_E_STATE; }
+  const int rc = gz_collect(z, h_out, out_cap, out_n, reinterpret_cast<GzSegResult *>(segs));
+  if (rc == LB2_OK && stats) *stats = z->st;
+  return rc;
 }
 
 }  // extern "C"

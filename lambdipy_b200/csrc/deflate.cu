@@ -1,8 +1,10 @@
-// deflate.cu -- raw DEFLATE (RFC 1951) encoder and CRC-32 for the gzip writer (lb2_gzip_* in api.cu).
+// deflate.cu -- raw DEFLATE (RFC 1951) encoder and CRC-32 for the gzip and zip writers (lb2_gzip_* / lb2_zip_* in api.cu).
 //
-// One CTA deflates one GZ_CHUNK-byte chunk of a piece.  It may reference the GZ_HIST bytes before the chunk (also
-// bytes of the previous piece, which the host keeps in front of the piece on the device), so cutting the stream into
-// chunks costs almost nothing in ratio.  Per chunk:
+// One CTA deflates one chunk of a piece: <= GZ_CHUNK bytes of one segment (a gzip stream's piece or one zip member's
+// bytes), described by the chunk table.  It may reference the chunk's `hist` bytes in front of it, which belong to the
+// same segment or, for a piece's first segment, to the same stream or file in earlier pieces (the host keeps them in
+// front of the piece on the device), so cutting a stream into chunks costs almost nothing in ratio and no match ever
+// reaches into another file.  Per chunk:
 //   1. in sub-blocks of SUB positions: load the window [pos - 32 KB, sub-block end + 258) into shared memory, build
 //      hash chains over it (one warp, __match_any_sync per 32 positions), find each position's longest match among
 //      CHAIN candidates (all threads), then walk the sub-block with greedy + one-step lazy parsing (zlib's
@@ -11,9 +13,9 @@
 //      coding and keep the smallest;
 //   3. pack the tokens: bit offsets from a block-wide exclusive scan of the code lengths, bits ORed into disjoint
 //      ranges of a shared-memory buffer (deterministic); close with an empty stored block (Z_SYNC_FLUSH) so the
-//      chunk ends byte-aligned.
-// A second kernel computes per-chunk CRC-32s; a single-CTA kernel scans the chunk sizes and combines the CRCs
-// (GF(2) multiply by x^(8n), as zlib's crc32_combine), and a gather kernel compacts the chunk outputs.
+//      chunk ends byte-aligned, and, if the chunk ends a file, with the final block 03 00.
+// A second kernel computes per-chunk CRC-32s; a single-CTA kernel scans the chunk sizes and combines the CRCs of each
+// segment (GF(2) multiply by x^(8n), as zlib's crc32_combine), and a gather kernel compacts the chunk outputs.
 #include "lb2_common.cuh"
 #include "copy_device.cuh"
 
@@ -238,10 +240,9 @@ __global__ void __launch_bounds__(DF_THREADS, 1) lb2_deflate_kernel(GzPieceArgs 
   uint16_t *head = reinterpret_cast<uint16_t *>(rec);  // only while the chains are built
   __shared__ DfShared S;
   const int tid = threadIdx.x;
-  const uint64_t c0 = (uint64_t)blockIdx.x * GZ_CHUNK;
-  const uint32_t clen = (uint32_t)(a.n - c0 < GZ_CHUNK ? a.n - c0 : GZ_CHUNK);
-  const uint64_t before = c0 + a.hist;  // stream bytes that exist before the chunk
-  uint32_t *tok = a.tokens + (uint64_t)blockIdx.x * GZ_CHUNK;
+  // the chunk's fields are read where they are used rather than kept in registers through the match finding
+  const GzChunk *ch = a.chunks + blockIdx.x;
+  const uint32_t clen = ch->len;
 
   for (int i = tid; i < 288; i += DF_THREADS) S.lfreq[i] = 0;
   if (tid < 32) S.dfreq[tid] = 0;
@@ -250,11 +251,11 @@ __global__ void __launch_bounds__(DF_THREADS, 1) lb2_deflate_kernel(GzPieceArgs 
   // ---- 1. match finding and parse, SUB positions per pass ------------------------------------------------
   uint32_t q = 0;
   while (q < clen) {
-    const uint32_t back = (uint32_t)(before + q < GZ_HIST ? before + q : GZ_HIST);
+    const uint32_t hist = ch->hist, back = hist + q < GZ_HIST ? hist + q : GZ_HIST;
     const uint32_t sub_end = q + SUB < clen ? q + SUB : clen;
     const uint32_t we = sub_end + 258 < clen ? sub_end + 258 : clen;  // matches end inside the chunk
     const uint32_t wlen = back + (we - q);
-    const uint8_t *src = a.in + c0 + q - back;
+    const uint8_t *src = a.in + ch->start + q - back;
     for (uint32_t i = tid; i < wlen; i += DF_THREADS) win[i] = src[i];
     for (uint32_t i = tid; i < (1u << HASH_BITS); i += DF_THREADS) head[i] = NIL;
     __syncthreads();
@@ -303,6 +304,7 @@ __global__ void __launch_bounds__(DF_THREADS, 1) lb2_deflate_kernel(GzPieceArgs 
     }
     __syncthreads();
     if (tid == 0) {  // greedy parse with one-step lazy evaluation
+      uint32_t *tok = a.tokens + ch->start;
       const uint32_t limit = sub_end < clen ? sub_end - 1 : clen;  // rec[p + 1] must be known
       uint32_t p = q, nt = S.ntok;
       while (p < limit) {
@@ -397,11 +399,16 @@ __global__ void __launch_bounds__(DF_THREADS, 1) lb2_deflate_kernel(GzPieceArgs 
     uint32_t mode = 0, size = stored_bytes;
     if (fix_bytes < size) { mode = 1; size = fix_bytes; }
     if (dyn_bytes < size) { mode = 2; size = dyn_bytes; }
+    if (clen == 0) size = 0;  // an empty file (stored was cheapest): no blocks, its body is the final block alone
     S.mode = mode; S.size = size; S.hclen = hclen; S.hdr_bits = mode == 2 ? hdr : 3;
   }
   __syncthreads();
   const uint32_t mode = S.mode, size = S.size;
-  uint8_t *out = a.chunk_out + (uint64_t)blockIdx.x * GZ_CHUNK_OUT_CAP;
+  // the file ends with this chunk: the final block 03 00 follows its output
+  const uint32_t fin = ch->last ? 2 : 0;
+  const uint64_t c0 = ch->start;
+  uint8_t *out = a.chunk_out + c0 + (uint64_t)blockIdx.x * GZ_OUT_PAD;
+  const uint32_t *tok = a.tokens + c0;
 
   // ---- 3. output --------------------------------------------------------------------------------------------
   if (mode == 0) {  // stored blocks of <= 65535 bytes, then the empty one
@@ -415,6 +422,7 @@ __global__ void __launch_bounds__(DF_THREADS, 1) lb2_deflate_kernel(GzPieceArgs 
       out[at + 1] = (uint8_t)len; out[at + 2] = (uint8_t)(len >> 8);
       out[at + 3] = (uint8_t)~len; out[at + 4] = (uint8_t)(~len >> 8);
     }
+    if (fin && tid == 0) { out[size] = 0x03; out[size + 1] = 0x00; }
   } else {
     // The fixed literal/length code is the canonical code over all 288 lengths (RFC 1951 3.2.6): the length-8
     // symbols 286 and 287 rank before every length-9 symbol, so leaving them out would shift the codes of the
@@ -481,14 +489,15 @@ __global__ void __launch_bounds__(DF_THREADS, 1) lb2_deflate_kernel(GzPieceArgs 
       const uint32_t nbytes = (bitpos + 3 + 7) / 8;  // empty stored block: 3 zero bits, pad, 00 00 FF FF
       uint8_t *b8 = reinterpret_cast<uint8_t *>(buf);
       b8[nbytes + 2] = 0xFF; b8[nbytes + 3] = 0xFF;
+      if (fin) b8[size] = 0x03;  // b8[size + 1] is already 0
     }
     __syncthreads();
     uint32_t *o32 = reinterpret_cast<uint32_t *>(out);
-    for (uint32_t i = tid; i < (size + 3) / 4; i += DF_THREADS) o32[i] = buf[i];
+    for (uint32_t i = tid; i < (size + fin + 3) / 4; i += DF_THREADS) o32[i] = buf[i];
   }
   if (tid == 0) {
-    a.chunk_size[blockIdx.x] = size;
-    a.chunk_mode[blockIdx.x] = mode;
+    a.chunk_size[blockIdx.x] = size + fin;
+    a.chunk_mode[blockIdx.x] = clen ? mode : 3;
   }
 }
 
@@ -525,8 +534,10 @@ __device__ uint32_t crc_combine(uint32_t crc_a, uint32_t crc_b, uint64_t len_b, 
   return multmodp(p, crc_a) ^ crc_b;
 }
 
-// CRC-32 of each GZ_CHUNK-byte chunk of in[0 .. n); in is 16-byte aligned
-__global__ void __launch_bounds__(CRC_THREADS) lb2_crc32_kernel(const uint8_t *in, uint64_t n, uint32_t *chunk_crc) {
+// CRC-32 of each chunk of the table (NULL: each GZ_CHUNK-byte chunk of in[0 .. n)); in and every chunk start are
+// 16-byte aligned
+__global__ void __launch_bounds__(CRC_THREADS) lb2_crc32_kernel(const uint8_t *in, uint64_t n, const GzChunk *chunks,
+                                                                uint32_t *chunk_crc) {
   __shared__ uint32_t tab[256], xt[32], s_crc[CRC_THREADS], s_len[CRC_THREADS];
   const int tid = threadIdx.x;
   {
@@ -536,9 +547,18 @@ __global__ void __launch_bounds__(CRC_THREADS) lb2_crc32_kernel(const uint8_t *i
   }
   if (tid == 0) init_x2n(xt);
   __syncthreads();
-  const uint64_t c0 = (uint64_t)blockIdx.x * GZ_CHUNK + (uint64_t)tid * CRC_SUB;
-  const uint32_t len = c0 >= n ? 0 : (uint32_t)(n - c0 < CRC_SUB ? n - c0 : CRC_SUB);
-  const uint8_t *p = in + c0;
+  uint64_t cs;
+  uint32_t cl;
+  if (chunks) {
+    cs = chunks[blockIdx.x].start;
+    cl = chunks[blockIdx.x].len;
+  } else {
+    cs = (uint64_t)blockIdx.x * GZ_CHUNK;
+    cl = (uint32_t)(n - cs < GZ_CHUNK ? n - cs : GZ_CHUNK);
+  }
+  const uint32_t o = (uint32_t)tid * CRC_SUB;
+  const uint32_t len = o >= cl ? 0 : (cl - o < CRC_SUB ? cl - o : CRC_SUB);
+  const uint8_t *p = in + cs + o;
   uint32_t crc = 0xFFFFFFFFu;
   uint32_t i = 0;
   for (; i + 16 <= len; i += 16) {  // sub-blocks are multiples of 16
@@ -564,26 +584,32 @@ __global__ void __launch_bounds__(CRC_THREADS) lb2_crc32_kernel(const uint8_t *i
 // ---- offsets, stream CRC, gather ---------------------------------------------------------------------------------
 constexpr int SCAN_THREADS = 1024;
 
+// Offsets of the chunk outputs in `out` and, per segment, its output range and CRC-32.  CRC-32 is linear: crc(c_1 .. c_k) = XOR over i of crc(c_i) * x^(8 L_i), L_i the
+// segment bytes after chunk i, so each chunk's term is computed on its own and XORed into its segment.
 __global__ void __launch_bounds__(SCAN_THREADS) lb2_gzip_scan_kernel(GzPieceArgs a) {
-  __shared__ unsigned long long s_sum[SCAN_THREADS], s_len[SCAN_THREADS];
-  __shared__ uint32_t s_crc[SCAN_THREADS], s_st[SCAN_THREADS], s_fx[SCAN_THREADS], xt[32];
+  __shared__ unsigned long long s_sum[SCAN_THREADS];
+  __shared__ uint32_t s_st[SCAN_THREADS], s_fx[SCAN_THREADS], xt[32];
   const int tid = threadIdx.x;
   if (tid == 0) init_x2n(xt);
+  const uint32_t per_s = (a.n_segs + SCAN_THREADS - 1) / SCAN_THREADS;
+  const uint32_t sb = min(a.n_segs, tid * per_s), se = min(a.n_segs, sb + per_s);
+  for (uint32_t s = sb; s < se; s++) a.seg_res[s].crc32 = 0;
   __syncthreads();
   const uint32_t per = (a.n_chunks + SCAN_THREADS - 1) / SCAN_THREADS;
   const uint32_t b = min(a.n_chunks, tid * per), e = min(a.n_chunks, b + per);
-  unsigned long long sum = 0, len = 0;
-  uint32_t crc = 0, st = 0, fx = 0;
+  unsigned long long sum = 0;
+  uint32_t st = 0, fx = 0;
   for (uint32_t i = b; i < e; i++) {
-    const uint64_t c0 = (uint64_t)i * GZ_CHUNK;
-    const uint64_t cl = a.n - c0 < GZ_CHUNK ? a.n - c0 : GZ_CHUNK;
+    const GzChunk c = a.chunks[i];
     sum += a.chunk_size[i];
     st += a.chunk_mode[i] == 0;
     fx += a.chunk_mode[i] == 1;
-    crc = crc_combine(crc, a.chunk_crc[i], cl, xt);
-    len += cl;
+    if (c.len) {
+      const GzSeg g = a.segs[c.seg];
+      atomicXor(&a.seg_res[c.seg].crc32, crc_combine(a.chunk_crc[i], 0, g.start + g.len - c.start - c.len, xt));
+    }
   }
-  s_sum[tid] = sum; s_len[tid] = len; s_crc[tid] = crc; s_st[tid] = st; s_fx[tid] = fx;
+  s_sum[tid] = sum; s_st[tid] = st; s_fx[tid] = fx;
   __syncthreads();
   for (int o = 1; o < SCAN_THREADS; o <<= 1) {  // inclusive scan of the output bytes
     const unsigned long long y = tid >= o ? s_sum[tid - o] : 0;
@@ -595,18 +621,29 @@ __global__ void __launch_bounds__(SCAN_THREADS) lb2_gzip_scan_kernel(GzPieceArgs
   for (uint32_t i = b; i < e; i++) { a.chunk_off[i] = off; off += a.chunk_size[i]; }
   for (int s = 1; s < SCAN_THREADS; s <<= 1) {
     if ((tid & (2 * s - 1)) == 0) {
-      s_crc[tid] = crc_combine(s_crc[tid], s_crc[tid + s], s_len[tid + s], xt);
-      s_len[tid] += s_len[tid + s];
       s_st[tid] += s_st[tid + s];
       s_fx[tid] += s_fx[tid + s];
     }
-    __syncthreads();
+    __syncthreads();  // also publishes chunk_off and the XORed segment CRCs to the whole block
   }
+  const unsigned long long total = s_sum[SCAN_THREADS - 1];
+  const uint32_t state = *a.crc_state;
+  for (uint32_t s = sb; s < se; s++) {
+    const GzSeg g = a.segs[s];
+    uint32_t crc = a.seg_res[s].crc32;
+    if (g.flags & GZ_SEG_CONTINUES) crc = crc_combine(state, crc, g.len, xt);
+    const unsigned long long o = a.chunk_off[g.first_chunk];
+    a.seg_res[s].out_off = o;
+    a.seg_res[s].out_len = (s + 1 < a.n_segs ? a.chunk_off[a.segs[s + 1].first_chunk] : total) - o;
+    a.seg_res[s].crc32 = crc;
+    a.seg_res[s].ended = (g.flags & GZ_SEG_ENDS) != 0;
+  }
+  __syncthreads();
   if (tid == 0) {
-    const uint32_t running = crc_combine(*a.crc_state, s_crc[0], a.n, xt);
+    const uint32_t running = a.segs[a.n_segs - 1].flags & GZ_SEG_ENDS ? 0u : a.seg_res[a.n_segs - 1].crc32;
     *a.crc_state = running;
     a.res->crc32 = running;
-    a.res->out_bytes = s_sum[SCAN_THREADS - 1];
+    a.res->out_bytes = total;
     a.res->n_stored = s_st[0];
     a.res->n_fixed = s_fx[0];
   }
@@ -646,7 +683,8 @@ __global__ void __launch_bounds__(SCAN_THREADS) lb2_crc32_combine_kernel(const u
 __global__ void __launch_bounds__(256) lb2_gzip_gather_kernel(GzPieceArgs a) {
   const uint32_t c = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (c >= a.n_chunks) return;
-  warp_copy_tile(a.chunk_out + (uint64_t)c * GZ_CHUNK_OUT_CAP, a.out + a.chunk_off[c], a.chunk_size[c], threadIdx.x & 31);
+  const int lane = threadIdx.x & 31;
+  warp_copy_tile(a.chunk_out + a.chunks[c].start + (uint64_t)c * GZ_OUT_PAD, a.out + a.chunk_off[c], a.chunk_size[c], lane);
 }
 
 }  // namespace
@@ -655,13 +693,15 @@ void launch_deflate(const GzPieceArgs &a, cudaStream_t s) {
   cudaFuncSetAttribute(lb2_deflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM);
   lb2_deflate_kernel<<<a.n_chunks, DF_THREADS, DF_DYN_SMEM, s>>>(a);
 }
-void launch_crc32(const GzPieceArgs &a, cudaStream_t s) { lb2_crc32_kernel<<<a.n_chunks, CRC_THREADS, 0, s>>>(a.in, a.n, a.chunk_crc); }
+void launch_crc32(const GzPieceArgs &a, cudaStream_t s) {
+  lb2_crc32_kernel<<<a.n_chunks, CRC_THREADS, 0, s>>>(a.in, a.n, a.chunks, a.chunk_crc);
+}
 void launch_crc32(const uint8_t *in, uint64_t n, uint32_t *chunk_crc, uint32_t *crc, cudaStream_t s) {
   if (!n) {
     cudaMemsetAsync(crc, 0, sizeof(uint32_t), s);
     return;
   }
-  lb2_crc32_kernel<<<(unsigned)((n + GZ_CHUNK - 1) / GZ_CHUNK), CRC_THREADS, 0, s>>>(in, n, chunk_crc);
+  lb2_crc32_kernel<<<(unsigned)((n + GZ_CHUNK - 1) / GZ_CHUNK), CRC_THREADS, 0, s>>>(in, n, nullptr, chunk_crc);
   lb2_crc32_combine_kernel<<<1, SCAN_THREADS, 0, s>>>(chunk_crc, n, crc);
 }
 void launch_gzip_compact(const GzPieceArgs &a, cudaStream_t s) {

@@ -135,15 +135,21 @@ def strip_build_tree(build_directory, backend=None, cleanup=False, keep_tests=No
 LAMBDA_UNZIPPED_LIMIT = 250 * 1024 * 1024  # the limit the reference exists to meet (/root/reference/README.md:4-5)
 
 
-def bundle_report(build_directory):
-    """Size of the finished bundle against Lambda's 250 MB unzipped limit (the reference's README
-    promises 'tips to further improve your bundle size' as a TODO, README.md:23)."""
+def tree_bytes(build_directory):
+    """bytes of the regular files under build_directory (symlinks not counted)"""
     total = 0
     for d, _, fs in os.walk(build_directory):
         for f in fs:
             p = os.path.join(d, f)
             if not os.path.islink(p):
                 total += os.path.getsize(p)
+    return total
+
+
+def bundle_report(build_directory):
+    """Size of the finished bundle against Lambda's 250 MB unzipped limit (the reference's README
+    promises 'tips to further improve your bundle size' as a TODO, README.md:23)."""
+    total = tree_bytes(build_directory)
     pct = 100.0 * total / LAMBDA_UNZIPPED_LIMIT
     return "Bundle size: %.1f MB = %.0f %% of the 250 MB Lambda limit%s" % (total / 1e6, pct, "" if pct <= 100 else "  ** over the limit **")
 
