@@ -218,6 +218,16 @@ int lb2_corpus_scatter(lb2_ctx *ctx, void *d_arena, const void *h_data, uint64_t
  * stored blocks, whichever is smallest, so incompressible data grows by at most LB2_GZIP_BOUND.
  * The same stream always gives the same bytes.
  *
+ * Modes (flags of lb2_gzip_create and lb2_zip_create).  0: each chunk is parsed greedily with one-step lazy
+ * evaluation over 16 hash-chain candidates per position.  LB2_DEFLATE_BEST: the thorough mode, for archives that are
+ * written once and downloaded many times.  After that parse, every chunk is parsed again optimally: each position's
+ * Pareto set of matches (up to 8, from up to 1024 hash-chain candidates) and a shortest path over the chunk's
+ * positions, priced with the chunk's own Huffman code, four rounds of parse -> code -> prices.  A chunk keeps the
+ * smaller of the two parses by the same byte formula, so a best-mode chunk is never larger than the default one; the
+ * chunking, flushes, bounds and determinism are those of mode 0.  A best-mode writer holds one workspace of
+ * 64 KB x 9 x 4 B = 2.25 MiB per SM of the device (297 MiB on a 132-SM H100) from create to destroy, beside the
+ * per-piece buffers both modes hold.
+ *
  * Up to TWO pieces may be in flight: lb2_gzip_submit enqueues the upload and the kernels and returns;
  * lb2_gzip_collect waits for the OLDEST piece and copies its compressed bytes out.  h_in must stay
  * unchanged until its piece is collected (pinned memory from lb2_pinned_alloc makes the upload
@@ -232,10 +242,13 @@ typedef struct lb2_gzip_stats {
   float crc_ms;                      /* CRC-32 kernel                                                 */
   float h2d_ms;                      /* piece uploads (CUDA events)                                   */
   float d2h_ms;                      /* result downloads (host clock around the copy)                 */
+  uint32_t n_opt_chunks;             /* chunks written from the optimal parse (0 in the default mode) */
+  float best_ms;                     /* best mode: the optimal-parse kernel (also in deflate_ms)      */
 } lb2_gzip_stats;
+#define LB2_DEFLATE_BEST 1u          /* lb2_gzip_create / lb2_zip_create: the thorough mode (above)   */
 /* worst-case DEFLATE bytes of one piece of n input bytes (out_cap of lb2_gzip_collect) */
 #define LB2_GZIP_BOUND(n) ((n) + 15 * (((n) + 65535) / 65536))
-int lb2_gzip_create(lb2_ctx *ctx, uint32_t flags /* 0 */, lb2_gzip **g);
+int lb2_gzip_create(lb2_ctx *ctx, uint32_t flags /* 0 or LB2_DEFLATE_BEST */, lb2_gzip **g);
 int lb2_gzip_submit(lb2_gzip *g, const void *h_in, uint64_t n);
 /* LB2_E_CAPACITY when out_cap is too small: *out_n says how much is needed, the piece stays in flight */
 int lb2_gzip_collect(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n);
@@ -253,7 +266,8 @@ void lb2_gzip_destroy(lb2_gzip *g);
  * + seg_len[i]), seg_off[i] a multiple of 16, in increasing order without overlap.  Each segment is deflated
  * like a gzip piece (64 KB chunks, sync-flushed, dynamic / fixed / stored per chunk), but no chunk crosses a
  * segment and no match reaches into another file; a file that ends in the piece is closed with the 2-byte final
- * block 03 00, so an empty file's body is exactly 03 00 (as zlib's).  Each member costs at most 5 + 2 bytes of
+ * block 03 00, so an empty file's body is exactly 03 00 (as zlib's); flags select the mode, as for lb2_gzip_create.
+ * Each member costs at most 5 + 2 bytes of
  * framing per 64 KB chunk, plus 2 for its final block, over its stored size.
  *
  * A file larger than a piece continues into the next one: submit its first part as the LAST segment with
@@ -278,7 +292,7 @@ typedef struct lb2_zip_segment {
 #define LB2_ZIP_MORE      2u   /* the last segment's file continues in the next piece                       */
 /* worst-case DEFLATE bytes of one piece of n bytes (padding included) in n_segs segments (out_cap of lb2_zip_collect) */
 #define LB2_ZIP_BOUND(n, n_segs) (LB2_GZIP_BOUND(n) + 17 * (uint64_t)(n_segs))
-int lb2_zip_create(lb2_ctx *ctx, uint32_t flags /* 0 */, lb2_zip **z);
+int lb2_zip_create(lb2_ctx *ctx, uint32_t flags /* 0 or LB2_DEFLATE_BEST */, lb2_zip **z);
 /* LB2_E_STATE: two pieces in flight, LB2_ZIP_CONTINUES without an open file, or an open file not continued */
 int lb2_zip_submit(lb2_zip *z, const void *h_in, uint64_t n, const uint64_t *seg_off, const uint64_t *seg_len,
                    uint32_t n_segs, uint32_t flags);

@@ -29,6 +29,17 @@ EXPORTS = [
     "lb2_zip_create", "lb2_zip_submit", "lb2_zip_collect", "lb2_zip_destroy",
 ]
 ZIP_CONTINUES, ZIP_MORE = 1, 2
+DEFLATE_BEST = 1  # LB2_DEFLATE_BEST
+
+
+def deflate_flags(compresslevel):
+    """The lb2_gzip_create / lb2_zip_create flags of a writer's `compresslevel`: None keeps the default encoder, 9
+    selects the thorough mode (LB2_DEFLATE_BEST, an optimal parse).  There are no levels 1-8."""
+    if compresslevel is None:
+        return 0
+    if type(compresslevel) is int and compresslevel == 9:
+        return DEFLATE_BEST
+    raise ValueError("compresslevel=%r: expected None (the default encoder) or 9 (the optimal parse)" % (compresslevel,))
 
 
 def gzip_bound(n):
@@ -69,7 +80,7 @@ class GzipStats(C.Structure):
     _fields_ = [
         ("in_bytes", C.c_uint64), ("out_bytes", C.c_uint64), ("crc32", C.c_uint32), ("n_chunks", C.c_uint32),
         ("n_stored_chunks", C.c_uint32), ("n_fixed_chunks", C.c_uint32), ("deflate_ms", C.c_float), ("crc_ms", C.c_float), ("h2d_ms", C.c_float),
-        ("d2h_ms", C.c_float),
+        ("d2h_ms", C.c_float), ("n_opt_chunks", C.c_uint32), ("best_ms", C.c_float),
     ]
 
     def as_dict(self):

@@ -487,7 +487,7 @@ struct GzSlot {
   GzResult *d_res = nullptr, *h_res = nullptr;
   uint64_t cap_bytes = 0, cap_tab = 0;
   uint32_t cap_chunks = 0, cap_segs = 0;
-  cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // upload | deflate | crc | compact |
+  cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // upload | deflate | best | crc | compact |
   cudaEvent_t done = nullptr;
   uint32_t n_segs = 0;
 };
@@ -499,6 +499,8 @@ struct GzWriter {
   uint32_t *d_crc = nullptr;   // running CRC-32 of the open stream / file, advanced by each piece's scan kernel
   uint64_t hist_len = 0;
   bool open = false;           // the last piece submitted left a file open (zip)
+  uint32_t *d_best = nullptr;  // LB2_DEFLATE_BEST: best_slots workspace slots of BEST_WS_WORDS words, then the claim counter
+  uint32_t best_slots = 0;     // 0: default mode
   GzSlot slot[2];
   int head = 0, count = 0;     // pieces in flight, collected in submission order
   bool finished = false;
@@ -561,11 +563,17 @@ static int gz_slot_reserve(lb2_ctx *ctx, GzSlot &s, uint64_t n, uint32_t n_chunk
   return LB2_OK;
 }
 
-static int gz_create(lb2_ctx *ctx, GzWriter *g, const char *what) {
+static int gz_create(lb2_ctx *ctx, GzWriter *g, uint32_t flags, const char *what) {
   g->ctx = ctx;
   CK(cudaSetDevice(ctx->device));
-  cudaError_t e;
-  if ((e = cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking)) != cudaSuccess ||
+  cudaError_t e = cudaSuccess;
+  if (flags & LB2_DEFLATE_BEST) {  // one workspace slot per CTA the best-mode kernel keeps resident: one per SM
+    int sms = 0;
+    if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device)) == cudaSuccess)
+      e = cudaMalloc(&g->d_best, (uint64_t)sms * BEST_WS_WORDS * sizeof(uint32_t) + 16);
+    g->best_slots = e == cudaSuccess ? (uint32_t)sms : 0;
+  }
+  if (e != cudaSuccess || (e = cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking)) != cudaSuccess ||
       (e = cudaMalloc(&g->d_hist, GZ_HIST)) != cudaSuccess || (e = cudaMalloc(&g->d_crc, sizeof(uint32_t))) != cudaSuccess ||
       (e = cudaMemsetAsync(g->d_crc, 0, sizeof(uint32_t), g->stream)) != cudaSuccess) {
     ctx->err = std::string(what) + ": " + cudaGetErrorString(e);
@@ -580,6 +588,7 @@ static void gz_destroy(GzWriter *g) {
   for (auto &s : g->slot) gz_slot_free(s);
   cudaFree(g->d_hist);
   cudaFree(g->d_crc);
+  cudaFree(g->d_best);
   if (g->stream) cudaStreamDestroy(g->stream);
 }
 
@@ -619,6 +628,8 @@ static int gz_submit(GzWriter *g, const void *h_in, uint64_t n, const uint64_t *
   a.tokens = s.d_tok; a.chunk_out = s.d_chunk_out;
   a.chunk_size = s.d_meta; a.chunk_mode = s.d_meta + c; a.chunk_crc = s.d_meta + 2 * c;
   a.chunk_off = s.d_off; a.out = s.d_out; a.crc_state = g->d_crc; a.seg_res = s.d_seg; a.res = s.d_res;
+  a.best_ws = g->d_best; a.best_claim = g->d_best ? g->d_best + (uint64_t)g->best_slots * BEST_WS_WORDS : nullptr;
+  a.best_slots = g->best_slots;
   CK(cudaEventRecord(s.ev[0], st));
   if (cont && g->hist_len)
     CK(cudaMemcpyAsync(s.d_in + GZ_HIST - g->hist_len, g->d_hist, g->hist_len, cudaMemcpyDeviceToDevice, st));
@@ -627,10 +638,12 @@ static int gz_submit(GzWriter *g, const void *h_in, uint64_t n, const uint64_t *
   CK(cudaEventRecord(s.ev[1], st));
   launch_deflate(a, st);
   CK(cudaEventRecord(s.ev[2], st));
-  launch_crc32(a, st);
+  if (g->best_slots) launch_deflate_best(a, st);
   CK(cudaEventRecord(s.ev[3], st));
-  launch_gzip_compact(a, st);
+  launch_crc32(a, st);
   CK(cudaEventRecord(s.ev[4], st));
+  launch_gzip_compact(a, st);
+  CK(cudaEventRecord(s.ev[5], st));
   CK(cudaMemcpyAsync(s.h_res, s.d_res, sizeof(GzResult), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(s.h_seg, s.d_seg, n_segs * sizeof(GzSegResult), cudaMemcpyDeviceToHost, st));
   CK(cudaEventRecord(s.done, st));
@@ -669,11 +682,13 @@ static int gz_collect(GzWriter *g, void *h_out, uint64_t out_cap, uint64_t *out_
     float ms = 0;
     CK(cudaEventElapsedTime(&ms, s.ev[0], s.ev[1])); g->st.h2d_ms += ms;
     CK(cudaEventElapsedTime(&ms, s.ev[1], s.ev[2])); g->st.deflate_ms += ms;
-    CK(cudaEventElapsedTime(&ms, s.ev[3], s.ev[4])); g->st.deflate_ms += ms;
-    CK(cudaEventElapsedTime(&ms, s.ev[2], s.ev[3])); g->st.crc_ms += ms;
+    CK(cudaEventElapsedTime(&ms, s.ev[2], s.ev[3])); g->st.deflate_ms += ms; g->st.best_ms += ms;
+    CK(cudaEventElapsedTime(&ms, s.ev[4], s.ev[5])); g->st.deflate_ms += ms;
+    CK(cudaEventElapsedTime(&ms, s.ev[3], s.ev[4])); g->st.crc_ms += ms;
     g->st.crc32 = s.h_res->crc32;
     g->st.n_stored_chunks += s.h_res->n_stored;
     g->st.n_fixed_chunks += s.h_res->n_fixed;
+    g->st.n_opt_chunks += s.h_res->n_opt;
     g->st.out_bytes += total;
     if (segs) std::copy(s.h_seg, s.h_seg + s.n_segs, segs);
   }
@@ -689,9 +704,9 @@ extern "C" {
 int lb2_gzip_create(lb2_ctx *ctx, uint32_t flags, lb2_gzip **out) {
   if (!ctx || !out) { if (ctx) ctx->err = "NULL argument"; return LB2_E_ARG; }
   *out = nullptr;
-  if (flags) { ctx->err = "lb2_gzip_create: no flags are defined"; return LB2_E_ARG; }
+  if (flags & ~LB2_DEFLATE_BEST) { ctx->err = "lb2_gzip_create: unknown flags"; return LB2_E_ARG; }
   lb2_gzip *g = new lb2_gzip();
-  const int rc = gz_create(ctx, g, "lb2_gzip_create");
+  const int rc = gz_create(ctx, g, flags, "lb2_gzip_create");
   if (rc) { lb2_gzip_destroy(g); return rc; }
   *out = g;
   return LB2_OK;
@@ -753,9 +768,9 @@ static_assert(sizeof(GzSegResult) == sizeof(lb2_zip_segment), "the scan kernel w
 int lb2_zip_create(lb2_ctx *ctx, uint32_t flags, lb2_zip **out) {
   if (!ctx || !out) { if (ctx) ctx->err = "NULL argument"; return LB2_E_ARG; }
   *out = nullptr;
-  if (flags) { ctx->err = "lb2_zip_create: no flags are defined"; return LB2_E_ARG; }
+  if (flags & ~LB2_DEFLATE_BEST) { ctx->err = "lb2_zip_create: unknown flags"; return LB2_E_ARG; }
   lb2_zip *z = new lb2_zip();
-  const int rc = gz_create(ctx, z, "lb2_zip_create");
+  const int rc = gz_create(ctx, z, flags, "lb2_zip_create");
   if (rc) { lb2_zip_destroy(z); return rc; }
   *out = z;
   return LB2_OK;

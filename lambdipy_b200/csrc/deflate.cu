@@ -14,10 +14,13 @@
 //   3. pack the tokens: bit offsets from a block-wide exclusive scan of the code lengths, bits ORed into disjoint
 //      ranges of a shared-memory buffer (deterministic); close with an empty stored block (Z_SYNC_FLUSH) so the
 //      chunk ends byte-aligned, and, if the chunk ends a file, with the final block 03 00.
+// In best mode (LB2_DEFLATE_BEST) lb2_deflate_best_kernel then parses every chunk again optimally and rewrites it where
+// that is smaller (phases 2 and 3 are shared; the parse itself is in deflate_parse.cuh).
 // A second kernel computes per-chunk CRC-32s; a single-CTA kernel scans the chunk sizes and combines the CRCs of each
 // segment (GF(2) multiply by x^(8n), as zlib's crc32_combine), and a gather kernel compacts the chunk outputs.
 #include "lb2_common.cuh"
 #include "copy_device.cuh"
+#include "deflate_parse.cuh"
 
 namespace lb2 {
 namespace {
@@ -49,20 +52,10 @@ __constant__ uint16_t c_dbase[30] = {1, 2, 3, 4, 5, 7, 9, 13, 17, 25, 33, 49, 65
 __constant__ uint8_t c_dext[30] = {0, 0, 0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 5, 5, 6, 6, 7, 7, 8, 8, 9, 9, 10, 10, 11, 11, 12, 12, 13, 13};
 __constant__ uint8_t c_clorder[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5, 11, 4, 12, 3, 13, 2, 14, 1, 15};
 
-__device__ __forceinline__ uint32_t len_sym(uint32_t len) {  // 3..258 -> 257..285
-  if (len == 258) return 285;
-  const uint32_t l = len - 3;
-  if (l < 8) return 257 + l;
-  const uint32_t n = 31 - __clz(l);
-  return 257 + 4 * (n - 1) + ((l >> (n - 2)) & 3);
-}
-__device__ __forceinline__ uint32_t dist_sym(uint32_t d0) {  // distance - 1 -> 0..29
-  if (d0 < 4) return d0;
-  const uint32_t n = 31 - __clz(d0);
-  return 2 * n + ((d0 >> (n - 1)) & 1);
-}
-__device__ __forceinline__ uint32_t lext_bits(uint32_t sym) { return sym >= 265 && sym < 285 ? (sym - 261) / 4 : 0; }
-__device__ __forceinline__ uint32_t dext_bits(uint32_t sym) { return sym >= 4 ? sym / 2 - 1 : 0; }
+using dp::dext_bits;
+using dp::dist_sym;
+using dp::len_sym;
+using dp::lext_bits;
 
 __device__ __forceinline__ uint32_t hash3(const uint8_t *w, uint32_t i) {
   const uint32_t v = (uint32_t)w[i] | ((uint32_t)w[i + 1] << 8) | ((uint32_t)w[i + 2] << 16);
@@ -232,106 +225,36 @@ __device__ __forceinline__ void put_bits(uint32_t *buf, uint32_t &pos, uint32_t 
   pos += n;
 }
 
-__global__ void __launch_bounds__(DF_THREADS, 1) lb2_deflate_kernel(GzPieceArgs a) {
-  extern __shared__ __align__(16) uint8_t smem[];
-  uint8_t *win = smem;
-  uint16_t *prev = reinterpret_cast<uint16_t *>(smem + WIN_BYTES);
-  uint32_t *rec = reinterpret_cast<uint32_t *>(smem + WIN_BYTES + PREV_BYTES);
-  uint16_t *head = reinterpret_cast<uint16_t *>(rec);  // only while the chains are built
-  __shared__ DfShared S;
-  const int tid = threadIdx.x;
-  // the chunk's fields are read where they are used rather than kept in registers through the match finding
-  const GzChunk *ch = a.chunks + blockIdx.x;
-  const uint32_t clen = ch->len;
-
-  for (int i = tid; i < 288; i += DF_THREADS) S.lfreq[i] = 0;
-  if (tid < 32) S.dfreq[tid] = 0;
-  if (tid == 0) S.ntok = 0;
-
-  // ---- 1. match finding and parse, SUB positions per pass ------------------------------------------------
-  uint32_t q = 0;
-  while (q < clen) {
-    const uint32_t hist = ch->hist, back = hist + q < GZ_HIST ? hist + q : GZ_HIST;
-    const uint32_t sub_end = q + SUB < clen ? q + SUB : clen;
-    const uint32_t we = sub_end + 258 < clen ? sub_end + 258 : clen;  // matches end inside the chunk
-    const uint32_t wlen = back + (we - q);
-    const uint8_t *src = a.in + ch->start + q - back;
-    for (uint32_t i = tid; i < wlen; i += DF_THREADS) win[i] = src[i];
-    for (uint32_t i = tid; i < (1u << HASH_BITS); i += DF_THREADS) head[i] = NIL;
-    __syncthreads();
-    const uint32_t nh = wlen >= 3 ? wlen - 2 : 0;
-    if (tid < 32) {  // prev[i]: the nearest earlier window position with the same hash
-      const int lane = tid;
-      for (uint32_t base = 0; base < nh; base += 32) {
-        const uint32_t i = base + lane;
-        const bool v = i < nh;
-        const uint32_t h = v ? hash3(win, i) : 0x80000000u + lane;
-        const unsigned grp = __match_any_sync(0xffffffffu, h);
-        const unsigned lower = grp & ((1u << lane) - 1);
-        uint16_t p = NIL;
-        if (lower) p = (uint16_t)(base + 31 - __clz(lower));
-        else if (v) p = head[h];
-        __syncwarp();
-        if (v) {
-          prev[i] = p;
-          if ((grp >> lane) == 1u) head[h] = (uint16_t)i;
-        }
-        __syncwarp();
+// prev[i]: the nearest earlier position of the window win[0 .. wlen) with the same hash (warp 0; head: the
+// 1 << HASH_BITS chain heads, NIL)
+__device__ __forceinline__ void build_chains(const uint8_t *win, uint32_t wlen, uint16_t *prev, uint16_t *head) {
+  const uint32_t nh = wlen >= 3 ? wlen - 2 : 0;
+  if (threadIdx.x < 32) {
+    const int lane = threadIdx.x;
+    for (uint32_t base = 0; base < nh; base += 32) {
+      const uint32_t i = base + lane;
+      const bool v = i < nh;
+      const uint32_t h = v ? hash3(win, i) : 0x80000000u + lane;
+      const unsigned grp = __match_any_sync(0xffffffffu, h);
+      const unsigned lower = grp & ((1u << lane) - 1);
+      uint16_t p = NIL;
+      if (lower) p = (uint16_t)(base + 31 - __clz(lower));
+      else if (v) p = head[h];
+      __syncwarp();
+      if (v) {
+        prev[i] = p;
+        if ((grp >> lane) == 1u) head[h] = (uint16_t)i;
       }
+      __syncwarp();
     }
-    __syncthreads();
-    const uint32_t np = sub_end - q;
-    for (uint32_t j = tid; j < np; j += DF_THREADS) {
-      const uint32_t c = back + j, pos = q + j;
-      const uint32_t max_len = clen - pos < 258 ? clen - pos : 258;
-      uint32_t best = 0, bdist = 0;
-      if (max_len >= 3) {
-        uint32_t cand = prev[c];
-        for (int k = 0; k < CHAIN && cand != NIL && c - cand <= 32768; k++) {
-          if (win[cand + best] == win[c + best]) {
-            const uint32_t l = match_len(win, c, cand, max_len);
-            if (l > best) {
-              best = l;
-              bdist = c - cand;
-              if (l >= NICE || l >= max_len) break;
-            }
-          }
-          cand = prev[cand];
-        }
-      }
-      if (best < 3 || (best == 3 && bdist > TOO_FAR)) best = 0;
-      rec[j] = best | (bdist << 16);
-    }
-    __syncthreads();
-    if (tid == 0) {  // greedy parse with one-step lazy evaluation
-      uint32_t *tok = a.tokens + ch->start;
-      const uint32_t limit = sub_end < clen ? sub_end - 1 : clen;  // rec[p + 1] must be known
-      uint32_t p = q, nt = S.ntok;
-      while (p < limit) {
-        const uint32_t r = rec[p - q];
-        uint32_t l = r & 0x1FF;
-        if (l >= 3 && l < LAZY_MAX && p + 1 < clen && (rec[p + 1 - q] & 0x1FF) > l) l = 0;
-        if (l >= 3) {
-          const uint32_t d = r >> 16;
-          tok[nt++] = 0x80000000u | ((l - 3) << 16) | (d - 1);
-          S.lfreq[len_sym(l)]++;
-          S.dfreq[dist_sym(d - 1)]++;
-          p += l;
-        } else {
-          const uint32_t b = win[back + p - q];
-          tok[nt++] = b;
-          S.lfreq[b]++;
-          p++;
-        }
-      }
-      S.ntok = nt;
-      S.q = p;
-    }
-    __syncthreads();
-    q = S.q;
   }
+}
 
-  // ---- 2. codes and the cheapest block type ---------------------------------------------------------------
+// Phase 2: code lengths for S.lfreq / S.dfreq (S.lfreq[256] is set to 1, the end of block) and the cheapest block
+// type; S.mode (0 stored, 1 fixed, 2 dynamic) and S.size (bytes, sync flush included, final block not) get the
+// choice.  Whole block.
+__device__ __forceinline__ void choose_block(DfShared &S, uint32_t clen) {
+  const int tid = threadIdx.x;
   if (tid == 0) {
     S.lfreq[256] = 1;  // end of block
     int nz = 0;        // a distance tree needs two codes (one-code trees are incomplete; zlib does the same)
@@ -403,14 +326,21 @@ __global__ void __launch_bounds__(DF_THREADS, 1) lb2_deflate_kernel(GzPieceArgs 
     S.mode = mode; S.size = size; S.hclen = hclen; S.hdr_bits = mode == 2 ? hdr : 3;
   }
   __syncthreads();
+}
+
+// Phase 3: chunk c (*ch, clen bytes) in the block type choose_block picked, from its S.ntok tokens at
+// a.tokens + ch->start, into its output slot; chunk_size[c] and chunk_mode[c] (| mode_flag) are set.  smem: the
+// kernel's dynamic shared memory, used as the packing buffer.  Whole block.
+__device__ __forceinline__ void emit_block(const GzPieceArgs &a, const GzChunk *ch, uint32_t c, uint32_t clen,
+                                           uint8_t *smem, DfShared &S, uint32_t mode_flag) {
+  const int tid = threadIdx.x;
   const uint32_t mode = S.mode, size = S.size;
   // the file ends with this chunk: the final block 03 00 follows its output
   const uint32_t fin = ch->last ? 2 : 0;
   const uint64_t c0 = ch->start;
-  uint8_t *out = a.chunk_out + c0 + (uint64_t)blockIdx.x * GZ_OUT_PAD;
+  uint8_t *out = a.chunk_out + c0 + (uint64_t)c * GZ_OUT_PAD;
   const uint32_t *tok = a.tokens + c0;
 
-  // ---- 3. output --------------------------------------------------------------------------------------------
   if (mode == 0) {  // stored blocks of <= 65535 bytes, then the empty one
     const uint8_t *in = a.in + c0;
     for (uint32_t i = tid; i < clen; i += DF_THREADS) out[i + 5 * (i / 65535 + 1)] = in[i];
@@ -496,8 +426,312 @@ __global__ void __launch_bounds__(DF_THREADS, 1) lb2_deflate_kernel(GzPieceArgs 
     for (uint32_t i = tid; i < (size + fin + 3) / 4; i += DF_THREADS) o32[i] = buf[i];
   }
   if (tid == 0) {
-    a.chunk_size[blockIdx.x] = size + fin;
-    a.chunk_mode[blockIdx.x] = clen ? mode : 3;
+    a.chunk_size[c] = size + fin;
+    a.chunk_mode[c] = clen ? mode | mode_flag : 3;
+  }
+}
+
+__global__ void __launch_bounds__(DF_THREADS, 1) lb2_deflate_kernel(GzPieceArgs a) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  uint8_t *win = smem;
+  uint16_t *prev = reinterpret_cast<uint16_t *>(smem + WIN_BYTES);
+  uint32_t *rec = reinterpret_cast<uint32_t *>(smem + WIN_BYTES + PREV_BYTES);
+  uint16_t *head = reinterpret_cast<uint16_t *>(rec);  // only while the chains are built
+  __shared__ DfShared S;
+  const int tid = threadIdx.x;
+  // the chunk's fields are read where they are used rather than kept in registers through the match finding
+  const GzChunk *ch = a.chunks + blockIdx.x;
+  const uint32_t clen = ch->len;
+
+  for (int i = tid; i < 288; i += DF_THREADS) S.lfreq[i] = 0;
+  if (tid < 32) S.dfreq[tid] = 0;
+  if (tid == 0) S.ntok = 0;
+
+  // ---- 1. match finding and parse, SUB positions per pass ------------------------------------------------
+  uint32_t q = 0;
+  while (q < clen) {
+    const uint32_t hist = ch->hist, back = hist + q < GZ_HIST ? hist + q : GZ_HIST;
+    const uint32_t sub_end = q + SUB < clen ? q + SUB : clen;
+    const uint32_t we = sub_end + 258 < clen ? sub_end + 258 : clen;  // matches end inside the chunk
+    const uint32_t wlen = back + (we - q);
+    const uint8_t *src = a.in + ch->start + q - back;
+    for (uint32_t i = tid; i < wlen; i += DF_THREADS) win[i] = src[i];
+    for (uint32_t i = tid; i < (1u << HASH_BITS); i += DF_THREADS) head[i] = NIL;
+    __syncthreads();
+    build_chains(win, wlen, prev, head);
+    __syncthreads();
+    const uint32_t np = sub_end - q;
+    for (uint32_t j = tid; j < np; j += DF_THREADS) {
+      const uint32_t c = back + j, pos = q + j;
+      const uint32_t max_len = clen - pos < 258 ? clen - pos : 258;
+      uint32_t best = 0, bdist = 0;
+      if (max_len >= 3) {
+        uint32_t cand = prev[c];
+        for (int k = 0; k < CHAIN && cand != NIL && c - cand <= 32768; k++) {
+          if (win[cand + best] == win[c + best]) {
+            const uint32_t l = match_len(win, c, cand, max_len);
+            if (l > best) {
+              best = l;
+              bdist = c - cand;
+              if (l >= NICE || l >= max_len) break;
+            }
+          }
+          cand = prev[cand];
+        }
+      }
+      if (best < 3 || (best == 3 && bdist > TOO_FAR)) best = 0;
+      rec[j] = best | (bdist << 16);
+    }
+    __syncthreads();
+    if (tid == 0) {  // greedy parse with one-step lazy evaluation
+      uint32_t *tok = a.tokens + ch->start;
+      const uint32_t limit = sub_end < clen ? sub_end - 1 : clen;  // rec[p + 1] must be known
+      uint32_t p = q, nt = S.ntok;
+      while (p < limit) {
+        const uint32_t r = rec[p - q];
+        uint32_t l = r & 0x1FF;
+        if (l >= 3 && l < LAZY_MAX && p + 1 < clen && (rec[p + 1 - q] & 0x1FF) > l) l = 0;
+        if (l >= 3) {
+          const uint32_t d = r >> 16;
+          tok[nt++] = 0x80000000u | ((l - 3) << 16) | (d - 1);
+          S.lfreq[len_sym(l)]++;
+          S.dfreq[dist_sym(d - 1)]++;
+          p += l;
+        } else {
+          const uint32_t b = win[back + p - q];
+          tok[nt++] = b;
+          S.lfreq[b]++;
+          p++;
+        }
+      }
+      S.ntok = nt;
+      S.q = p;
+    }
+    __syncthreads();
+    q = S.q;
+  }
+
+  // ---- 2. codes and the cheapest block type; 3. output ------------------------------------------------------
+  choose_block(S, clen);
+  emit_block(a, ch, blockIdx.x, clen, smem, S, 0);
+}
+
+// ---- best mode (LB2_DEFLATE_BEST): an optimal parse after the greedy one ------------------------------------------
+// Runs after lb2_deflate_kernel, whose output every chunk keeps unless the optimal parse is smaller by the same byte
+// formula.  One CTA per chunk, chunks claimed from a counter; each CTA owns one workspace slot:
+//   1. the greedy tokens' frequencies give the first costs and the size to beat;
+//   2. per sub-block as in pass 1, every position's Pareto match list (deflate_parse.cuh) from up to BEST_CHAIN
+//      hash-chain candidates, dp::K words per position in the slot;
+//   3. BEST_ITERS times: the cheapest path under the current costs (warp 0, one position at a time, its lengths split
+//      over the lanes; the lengths of the edges in shared memory), traced back on one thread, its tokens gathered in
+//      order by the whole block into the slot; their code (choose_block) prices them and gives the next costs;
+//   4. the smallest of these parses, if it beats the greedy one, is written with emit_block.
+constexpr uint32_t BEST_CHAIN = 1024;  // hash-chain candidates per position
+constexpr uint32_t BEST_ITERS = 4;     // parse -> code -> costs rounds
+constexpr uint32_t BEST_UNUSED_BITS = 15;  // cost of a symbol the current code does not have
+constexpr uint32_t STEP_OFF = WIN_BYTES;   // u16 step[0 .. GZ_CHUNK] over prev / rec once the match lists are built
+constexpr uint32_t PAR_OFF = WIN_BYTES + PREV_BYTES + (1u << HASH_BITS) * 2;  // per-thread Pareto lists, after the heads
+static_assert(STEP_OFF + (GZ_CHUNK + 1) * 2 <= DF_DYN_SMEM, "edge lengths fit in the match-finding buffers");
+static_assert(PAR_OFF + dp::K * DF_THREADS * 4 <= DF_DYN_SMEM, "Pareto lists fit beside the hash heads");
+static_assert(BEST_WS_WORDS == GZ_CHUNK * (dp::K + 1), "slot: match lists, then candidate tokens");
+
+struct BestShared {
+  dp::Costs cost;
+  uint32_t ring[dp::RING];
+  uint32_t ent[32 * dp::K];  // the match lists of 32 positions, staged for warp 0
+  uint8_t byte[32];
+  uint32_t edc[dp::K];
+  uint32_t best_l[288], best_d[32];
+  uint32_t best_size, best_ntok, chunk;
+};
+
+// next round's costs from the code choose_block just built (the fixed code if it chose that)
+__device__ __forceinline__ void set_costs(const DfShared &S, dp::Costs &c) {
+  const bool fixed = S.mode == 1;
+  for (uint32_t l = threadIdx.x; l < 256 + 259 + 30; l += DF_THREADS) {
+    if (l < 256) {
+      const uint32_t b = fixed ? (l < 144 ? 8 : 9) : S.llen[l];
+      c.lit[l] = b ? b : BEST_UNUSED_BITS;
+    } else if (l < 256 + 259) {
+      const uint32_t len = l - 256;
+      if (len < 3) continue;
+      const uint32_t s = len_sym(len);
+      const uint32_t b = fixed ? (s < 280 ? 7 : 8) : S.llen[s];
+      c.len[len] = (b ? b : BEST_UNUSED_BITS) + lext_bits(s);
+    } else {
+      const uint32_t s = l - 256 - 259;
+      const uint32_t b = fixed ? 5 : S.dlen[s];
+      c.dist[s] = (b ? b : BEST_UNUSED_BITS) + dext_bits(s);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(DF_THREADS, 1) lb2_deflate_best_kernel(GzPieceArgs a) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  uint8_t *win = smem;
+  uint16_t *prev = reinterpret_cast<uint16_t *>(smem + WIN_BYTES);
+  uint16_t *head = reinterpret_cast<uint16_t *>(smem + WIN_BYTES + PREV_BYTES);
+  uint32_t *par = reinterpret_cast<uint32_t *>(smem + PAR_OFF);
+  uint16_t *step = reinterpret_cast<uint16_t *>(smem + STEP_OFF);
+  __shared__ DfShared S;
+  __shared__ BestShared B;
+  const int tid = threadIdx.x, lane = tid & 31;
+  uint32_t *list = a.best_ws + (uint64_t)blockIdx.x * BEST_WS_WORDS;  // dp::K words per position of the chunk
+  uint32_t *cand = list + GZ_CHUNK * dp::K;                           // the current round's tokens
+
+  for (;;) {
+    __syncthreads();
+    if (tid == 0) B.chunk = atomicAdd(a.best_claim, 1u);
+    __syncthreads();
+    const uint32_t c = B.chunk;
+    if (c >= a.n_chunks) return;
+    const GzChunk *ch = a.chunks + c;
+    const uint32_t clen = ch->len;
+    if (clen == 0) continue;
+    const uint8_t *in = a.in + ch->start;
+    uint32_t *tok = a.tokens + ch->start;
+
+    // ---- 1. the greedy parse: its tokens cover the chunk exactly, those after them are stale -----------------
+    for (int i = tid; i < 288; i += DF_THREADS) S.lfreq[i] = 0;
+    if (tid < 32) S.dfreq[tid] = 0;
+    __syncthreads();
+    for (uint32_t base = 0, done = 0; done < clen; base += DF_THREADS) {
+      const uint32_t t = base + tid;
+      const uint32_t tk = t < clen ? tok[t] : 0;
+      const uint32_t len = t < clen ? (tk & 0x80000000u ? ((tk >> 16) & 0xFF) + 3 : 1) : 0;
+      uint32_t total;
+      const uint32_t at = done + block_excl_scan(len, S.warp_tot, &total);
+      if (len && at < clen) {
+        if (len == 1) {
+          atomicAdd(&S.lfreq[tk], 1u);
+        } else {
+          atomicAdd(&S.lfreq[len_sym(len)], 1u);
+          atomicAdd(&S.dfreq[dist_sym(tk & 0x7FFF)], 1u);
+        }
+      }
+      done += total;
+    }
+    __syncthreads();
+    choose_block(S, clen);
+    if (tid == 0) B.best_size = S.size;
+    set_costs(S, B.cost);
+
+    // ---- 2. Pareto match lists ----------------------------------------------------------------------------------
+    for (uint32_t q = 0; q < clen; q += SUB) {
+      const uint32_t hist = ch->hist, back = hist + q < GZ_HIST ? hist + q : GZ_HIST;
+      const uint32_t sub_end = q + SUB < clen ? q + SUB : clen;
+      const uint32_t we = sub_end + 258 < clen ? sub_end + 258 : clen;
+      const uint32_t wlen = back + (we - q);
+      const uint8_t *src = in + q - back;
+      __syncthreads();
+      for (uint32_t i = tid; i < wlen; i += DF_THREADS) win[i] = src[i];
+      for (uint32_t i = tid; i < (1u << HASH_BITS); i += DF_THREADS) head[i] = NIL;
+      __syncthreads();
+      build_chains(win, wlen, prev, head);
+      __syncthreads();
+      for (uint32_t j = tid; j < sub_end - q; j += DF_THREADS) {
+        const uint32_t cp = back + j, pos = q + j;
+        const uint32_t max_len = clen - pos < 258 ? clen - pos : 258;
+        uint32_t n = 0, best = 2;
+        if (max_len >= 3) {
+          uint32_t cd = prev[cp];
+          for (uint32_t k = 0; k < BEST_CHAIN && cd != NIL && cp - cd <= 32768; k++) {
+            if (win[cd + best] == win[cp + best]) {
+              const uint32_t l = match_len(win, cp, cd, max_len);
+              if (dp::pareto_insert(par + tid, DF_THREADS, n, l, cp - cd)) {
+                best = l;
+                if (l >= max_len) break;
+              }
+            }
+            cd = prev[cd];
+          }
+        }
+        uint32_t *o = list + (uint64_t)pos * dp::K;
+#pragma unroll
+        for (uint32_t k = 0; k < dp::K; k++) o[k] = k < n ? par[k * DF_THREADS + tid] : 0u;
+      }
+    }
+    __syncthreads();
+
+    // ---- 3. parse -> code -> costs rounds --------------------------------------------------------------------------
+    bool improved = false;
+    for (uint32_t it = 0; it < BEST_ITERS; it++) {
+      if (tid < 32) {  // the cheapest path: positions in order, the lengths from one position across the lanes
+        for (uint32_t s = lane; s < dp::RING; s += 32) B.ring[s] = s ? dp::INF : 0u;
+        for (uint32_t i = 0; i < clen; i++) {
+          const uint32_t r = i & 31;
+          if (r == 0) {  // stage the next 32 positions' lists and bytes
+            __syncwarp();
+            const uint32_t *src = list + (uint64_t)i * dp::K;
+            const uint32_t nw = (clen - i < 32 ? clen - i : 32) * dp::K;
+#pragma unroll
+            for (uint32_t k = 0; k < dp::K; k++) {
+              const uint32_t w = k * 32 + lane;
+              B.ent[w] = w < nw ? src[w] : 0u;
+            }
+            B.byte[lane] = i + lane < clen ? in[i + lane] : 0;
+            __syncwarp();
+          }
+          const uint32_t *e = B.ent + r * dp::K;
+          const uint32_t ek = lane < (int)dp::K ? e[lane] : 0u;
+          if (lane < (int)dp::K) B.edc[lane] = ek ? dp::entry_cost(B.cost, ek) : 0u;
+          const uint32_t n = __popc(__ballot_sync(0xffffffffu, ek != 0));
+          __syncwarp();
+          const uint32_t ci = B.ring[i & (dp::RING - 1)];
+          dp::relax(i, ci, B.byte[r], e, B.edc, n, B.cost, B.ring, step, lane, 32);
+          __syncwarp();
+          if (lane == 0) B.ring[i & (dp::RING - 1)] = dp::INF;
+        }
+      }
+      __syncthreads();
+      if (tid == 0) S.ntok = dp::trace_back(step, clen);
+      for (int i = tid; i < 288; i += DF_THREADS) S.lfreq[i] = 0;
+      if (tid < 32) S.dfreq[tid] = 0;
+      __syncthreads();
+      // the path's tokens in order: the marked edge ends, compacted with a block-wide scan
+      for (uint32_t base = 0, nt = 0; base < clen; base += DF_THREADS) {
+        const uint32_t t = base + 1 + tid;
+        const uint32_t sv = t <= clen ? step[t] : 0u;
+        const bool on = (sv & dp::ON_PATH) != 0;
+        uint32_t total;
+        const uint32_t idx = nt + block_excl_scan(on, S.warp_tot, &total);
+        if (on) {
+          const uint32_t l = sv & 0x7FFF, s = t - l;
+          const uint32_t tk = dp::path_token(l, in[s], list + (uint64_t)s * dp::K, 1);
+          cand[idx] = tk;
+          if (l == 1) {
+            atomicAdd(&S.lfreq[tk], 1u);
+          } else {
+            atomicAdd(&S.lfreq[len_sym(l)], 1u);
+            atomicAdd(&S.dfreq[dist_sym(tk & 0x7FFF)], 1u);
+          }
+        }
+        nt += total;
+      }
+      __syncthreads();
+      choose_block(S, clen);
+      const bool better = S.size < B.best_size;
+      __syncthreads();
+      if (better) {  // the smallest round so far: keep its tokens and frequencies
+        improved = true;
+        for (uint32_t i = tid; i < S.ntok; i += DF_THREADS) tok[i] = cand[i];
+        for (int i = tid; i < 288; i += DF_THREADS) B.best_l[i] = S.lfreq[i];
+        if (tid < 32) B.best_d[tid] = S.dfreq[tid];
+        if (tid == 0) { B.best_size = S.size; B.best_ntok = S.ntok; }
+      }
+      set_costs(S, B.cost);
+      __syncthreads();
+    }
+
+    // ---- 4. output ------------------------------------------------------------------------------------------------
+    if (improved) {
+      for (int i = tid; i < 288; i += DF_THREADS) S.lfreq[i] = B.best_l[i];
+      if (tid < 32) S.dfreq[tid] = B.best_d[tid];
+      if (tid == 0) S.ntok = B.best_ntok;
+      __syncthreads();
+      choose_block(S, clen);
+      emit_block(a, ch, c, clen, smem, S, GZ_MODE_OPT);
+    }
   }
 }
 
@@ -588,7 +822,7 @@ constexpr int SCAN_THREADS = 1024;
 // segment bytes after chunk i, so each chunk's term is computed on its own and XORed into its segment.
 __global__ void __launch_bounds__(SCAN_THREADS) lb2_gzip_scan_kernel(GzPieceArgs a) {
   __shared__ unsigned long long s_sum[SCAN_THREADS];
-  __shared__ uint32_t s_st[SCAN_THREADS], s_fx[SCAN_THREADS], xt[32];
+  __shared__ uint32_t s_st[SCAN_THREADS], s_fx[SCAN_THREADS], s_op[SCAN_THREADS], xt[32];
   const int tid = threadIdx.x;
   if (tid == 0) init_x2n(xt);
   const uint32_t per_s = (a.n_segs + SCAN_THREADS - 1) / SCAN_THREADS;
@@ -598,18 +832,20 @@ __global__ void __launch_bounds__(SCAN_THREADS) lb2_gzip_scan_kernel(GzPieceArgs
   const uint32_t per = (a.n_chunks + SCAN_THREADS - 1) / SCAN_THREADS;
   const uint32_t b = min(a.n_chunks, tid * per), e = min(a.n_chunks, b + per);
   unsigned long long sum = 0;
-  uint32_t st = 0, fx = 0;
+  uint32_t st = 0, fx = 0, op = 0;
   for (uint32_t i = b; i < e; i++) {
     const GzChunk c = a.chunks[i];
+    const uint32_t m = a.chunk_mode[i];
     sum += a.chunk_size[i];
-    st += a.chunk_mode[i] == 0;
-    fx += a.chunk_mode[i] == 1;
+    st += (m & 3) == 0;
+    fx += (m & 3) == 1;
+    op += (m & GZ_MODE_OPT) != 0;
     if (c.len) {
       const GzSeg g = a.segs[c.seg];
       atomicXor(&a.seg_res[c.seg].crc32, crc_combine(a.chunk_crc[i], 0, g.start + g.len - c.start - c.len, xt));
     }
   }
-  s_sum[tid] = sum; s_st[tid] = st; s_fx[tid] = fx;
+  s_sum[tid] = sum; s_st[tid] = st; s_fx[tid] = fx; s_op[tid] = op;
   __syncthreads();
   for (int o = 1; o < SCAN_THREADS; o <<= 1) {  // inclusive scan of the output bytes
     const unsigned long long y = tid >= o ? s_sum[tid - o] : 0;
@@ -623,6 +859,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) lb2_gzip_scan_kernel(GzPieceArgs
     if ((tid & (2 * s - 1)) == 0) {
       s_st[tid] += s_st[tid + s];
       s_fx[tid] += s_fx[tid + s];
+      s_op[tid] += s_op[tid + s];
     }
     __syncthreads();  // also publishes chunk_off and the XORed segment CRCs to the whole block
   }
@@ -646,6 +883,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) lb2_gzip_scan_kernel(GzPieceArgs
     a.res->out_bytes = total;
     a.res->n_stored = s_st[0];
     a.res->n_fixed = s_fx[0];
+    a.res->n_opt = s_op[0];
   }
 }
 
@@ -692,6 +930,11 @@ __global__ void __launch_bounds__(256) lb2_gzip_gather_kernel(GzPieceArgs a) {
 void launch_deflate(const GzPieceArgs &a, cudaStream_t s) {
   cudaFuncSetAttribute(lb2_deflate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM);
   lb2_deflate_kernel<<<a.n_chunks, DF_THREADS, DF_DYN_SMEM, s>>>(a);
+}
+void launch_deflate_best(const GzPieceArgs &a, cudaStream_t s) {
+  cudaFuncSetAttribute(lb2_deflate_best_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_DYN_SMEM);
+  cudaMemsetAsync(a.best_claim, 0, sizeof(uint32_t), s);
+  lb2_deflate_best_kernel<<<a.n_chunks < a.best_slots ? a.n_chunks : a.best_slots, DF_THREADS, DF_DYN_SMEM, s>>>(a);
 }
 void launch_crc32(const GzPieceArgs &a, cudaStream_t s) {
   lb2_crc32_kernel<<<a.n_chunks, CRC_THREADS, 0, s>>>(a.in, a.n, a.chunks, a.chunk_crc);

@@ -15,6 +15,9 @@ With LAMBDIPY_BUNDLE_ZIP=<path>.zip (default: unset, nothing changes), `copy_inc
 last step of `lambdipy build` -- is wrapped: after the reference's copy, ./build is zipped on the GPU into <path>
 (zipfile_gpu.zip_tree, the archive shutil.make_archive writes) and one line reports the zip against Lambda's 50 MB
 direct-upload limit and the tree against its 250 MB unzipped limit.
+
+With LAMBDIPY_DEFLATE_LEVEL=9 (default: unset, the default encoder) the GPU tarball mirror and the bundle zip use
+the thorough encoder (an optimal parse; smaller output, longer kernels).  No other value is accepted.
 """
 import os
 import sys
@@ -34,12 +37,25 @@ def bundle_zip_path():
     return path
 
 
-def zip_after_copy(copy_include_paths, zip_path):
+def deflate_level():
+    """LAMBDIPY_DEFLATE_LEVEL, checked: None when unset, else 9."""
+    level = os.environ.get("LAMBDIPY_DEFLATE_LEVEL")
+    if level is None:
+        return None
+    if level != "9":
+        raise ValueError("LAMBDIPY_DEFLATE_LEVEL=%r: expected 9 (the optimal parse) or unset (the default encoder)" % level)
+    return 9
+
+
+def zip_after_copy(copy_include_paths, zip_path, compresslevel=None):
     """copy_include_paths followed by the bundle zip of its build directory and the size line."""
     def wrapped(include_paths, build_directory="./build"):
         copy_include_paths(include_paths, build_directory)
         from . import project_build, zipfile_gpu
-        zipfile_gpu.zip_tree(build_directory, zip_path)
+        if compresslevel is None:
+            zipfile_gpu.zip_tree(build_directory, zip_path)
+        else:
+            zipfile_gpu.zip_tree(build_directory, zip_path, compresslevel=compresslevel)
         zipped, unzipped = os.path.getsize(zip_path), project_build.tree_bytes(build_directory)
         print("Bundle zip: %s, %.1f MB = %.0f %% of the 50 MB direct-upload limit; unzipped %.1f MB = %.0f %% of 250 MB"
               % (zip_path, zipped / 1e6, 100.0 * zipped / LAMBDA_ZIPPED_LIMIT, unzipped / 1e6,
@@ -55,6 +71,7 @@ def apply():
     if untar not in UNTAR_BACKENDS:
         raise ValueError("LAMBDIPY_UNTAR_BACKEND=%r: expected one of %s" % (untar, ", ".join(UNTAR_BACKENDS)))
     zip_path = bundle_zip_path()
+    level = deflate_level()
     import lambdipy.cli as cli
     import lambdipy.project_build as ref
     from . import project_build as mine
@@ -63,12 +80,12 @@ def apply():
     if backend == "b200":
         import lambdipy.package_build as ref_pkg
         from . import tarball
-        ref_pkg.PackageBuild.create_compressed_tarball = tarball.create_compressed_tarball
+        ref_pkg.PackageBuild.create_compressed_tarball = tarball.tarball_method(level)
     if untar == "b200":
         from . import tarball
         ref.prepare_tarfile = tarball.prepare_tarfile
     if zip_path is not None:
-        cli.copy_include_paths = zip_after_copy(ref.copy_include_paths, zip_path)
+        cli.copy_include_paths = zip_after_copy(ref.copy_include_paths, zip_path, level)
     # `lambdipy build` spends seconds resolving, downloading and copying packages before it reaches the
     # strip step (cli.py:52-67): create the CUDA context behind that, not in front of the strip
     if os.environ.get("LAMBDIPY_B200_EAGER_WARMUP", "1") != "0":

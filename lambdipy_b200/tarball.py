@@ -45,21 +45,23 @@ class GpuGzipFile(io.BufferedIOBase):
     uncompressed bytes, as GzipFile's does (tarfile reads it when it opens the archive).
 
     ctx=None: the context the strip path has already warmed up in this process (project_build.warmup), if
-    any, else a new one on device LAMBDIPY_B200_DEVICE (default 0) that close() releases."""
+    any, else a new one on device LAMBDIPY_B200_DEVICE (default 0) that close() releases.
 
-    def __init__(self, filename, mtime=None, ctx=None, piece_bytes=PIECE_BYTES):
+    compresslevel=None keeps the default encoder; 9 selects the thorough one (LB2_DEFLATE_BEST: an optimal parse,
+    never larger, slower); anything else raises ValueError."""
+
+    def __init__(self, filename, mtime=None, ctx=None, piece_bytes=PIECE_BYTES, compresslevel=None):
         self.name = filename
         self._own_ctx = False
+        self._ctx = self._g = self._out = self._file = None
+        self._bufs = []
+        flags = N.deflate_flags(compresslevel)  # checked before anything is allocated
         if ctx is None:
             ctx, self._own_ctx = _default_context()
         self._ctx = ctx
-        self._g = None
-        self._bufs = []
-        self._out = None
-        self._file = None
         try:
             g = C.c_void_p()
-            self._ctx.check(self._ctx.lib.lb2_gzip_create(self._ctx.h, 0, C.byref(g)))
+            self._ctx.check(self._ctx.lib.lb2_gzip_create(self._ctx.h, flags, C.byref(g)))
             self._g = g
             self._piece = int(piece_bytes)
             for _ in range(2):
@@ -178,22 +180,39 @@ def gzip_header(filename, mtime=None):
     return head + (fname + b"\0" if fname else b"")
 
 
-def gzip_tarball(src_paths, tarball_path, ctx=None):
+def gzip_tarball(src_paths, tarball_path, ctx=None, compresslevel=None):
     """Write `tarball_path` as a gzip-compressed tar of `src_paths`, each added recursively under its
     basename -- what `tarfile.open(tarball_path, "w:gz")` with `tar.add(p, arcname=basename(p))` writes,
-    with the same tar stream.  Returns tarball_path."""
-    with GpuGzipFile(tarball_path, ctx=ctx) as gz, tarfile.open(name=tarball_path, mode="w", fileobj=gz) as tar:
+    with the same tar stream.  compresslevel: as GpuGzipFile's.  Returns tarball_path."""
+    N.deflate_flags(compresslevel)
+    with GpuGzipFile(tarball_path, ctx=ctx, compresslevel=compresslevel) as gz, tarfile.open(name=tarball_path, mode="w", fileobj=gz) as tar:
         for path in src_paths:
             tar.add(path, arcname=os.path.basename(path))
     return tarball_path
 
 
-def create_compressed_tarball(package_build, ctx=None):
+def create_compressed_tarball(package_build, ctx=None, compresslevel=None):
     """Mirror of PackageBuild.create_compressed_tarball: every top-level entry of the package's build
-    directory into ~/.lambdipy/build/<git tag>.tar.gz; returns that path."""
+    directory into ~/.lambdipy/build/<git tag>.tar.gz; returns that path.  compresslevel: as GpuGzipFile's."""
+    N.deflate_flags(compresslevel)
     home = os.environ["HOME"]
     tarball_path = f"{home}/.lambdipy/build/{package_build.git_tag()}.tar.gz"
-    return gzip_tarball(glob.glob(f"{package_build.build_directory()}/*"), tarball_path, ctx)
+    srcs = glob.glob(f"{package_build.build_directory()}/*")
+    if compresslevel is None:
+        return gzip_tarball(srcs, tarball_path, ctx)
+    return gzip_tarball(srcs, tarball_path, ctx, compresslevel=compresslevel)
+
+
+def tarball_method(compresslevel):
+    """The PackageBuild.create_compressed_tarball that patch.apply() installs: the mirror itself for the default
+    encoder, else the mirror writing at `compresslevel`."""
+    N.deflate_flags(compresslevel)
+    if compresslevel is None:
+        return create_compressed_tarball
+
+    def create_compressed_tarball_at_level(package_build):
+        return create_compressed_tarball(package_build, compresslevel=compresslevel)
+    return create_compressed_tarball_at_level
 
 
 # ---- reading ------------------------------------------------------------------------------------------------------

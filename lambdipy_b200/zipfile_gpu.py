@@ -36,14 +36,16 @@ class GpuZipEncoder:
 
     buffers[k]: writable memoryview of piece_bytes; submit(k, n, seg_off, seg_len, flags) hands buffers[k][:n] to the
     GPU (flags: N.ZIP_CONTINUES / N.ZIP_MORE); collect() waits for the oldest piece and returns (its DEFLATE bytes,
-    [(out_off, out_len, crc32, ended) per segment]); the bytes stay valid until the next collect()."""
+    [(out_off, out_len, crc32, ended) per segment]); the bytes stay valid until the next collect().
+    compresslevel: None (the default encoder) or 9 (the optimal parse, LB2_DEFLATE_BEST)."""
 
-    def __init__(self, ctx, piece_bytes=PIECE_BYTES, max_segs=MAX_SEGS):
+    def __init__(self, ctx, piece_bytes=PIECE_BYTES, max_segs=MAX_SEGS, compresslevel=None):
+        flags = N.deflate_flags(compresslevel)  # checked before anything is allocated
         self._ctx, self._z, self._ptrs, self._out = ctx, None, [], None
         self.piece_bytes, self.max_segs = int(piece_bytes), int(max_segs)
         try:
             z = C.c_void_p()
-            ctx.check(ctx.lib.lb2_zip_create(ctx.h, 0, C.byref(z)))
+            ctx.check(ctx.lib.lb2_zip_create(ctx.h, flags, C.byref(z)))
             self._z = z
             self.buffers = []
             for _ in range(2):
@@ -75,7 +77,8 @@ class GpuZipEncoder:
         st = self._stats
         return {"kernel_ms": st.deflate_ms + st.crc_ms, "deflate_ms": st.deflate_ms, "crc_ms": st.crc_ms,
                 "h2d_ms": st.h2d_ms, "d2h_ms": st.d2h_ms, "n_chunks": st.n_chunks,
-                "n_stored_chunks": st.n_stored_chunks, "n_fixed_chunks": st.n_fixed_chunks}
+                "n_stored_chunks": st.n_stored_chunks, "n_fixed_chunks": st.n_fixed_chunks,
+                "n_opt_chunks": st.n_opt_chunks, "best_ms": st.best_ms}
 
     def close(self):
         if self._z is not None:
@@ -279,18 +282,21 @@ def write_zip(root_dir, zip_path, encoder):
     return st
 
 
-def zip_tree(root_dir, zip_path, ctx=None, piece_bytes=PIECE_BYTES):
+def zip_tree(root_dir, zip_path, ctx=None, piece_bytes=PIECE_BYTES, compresslevel=None):
     """Write `zip_path` as `shutil.make_archive(zip_path[:-4], "zip", root_dir)` would, with every member's DEFLATE
     body and CRC-32 computed on the GPU.  Returns a stats dict: files, entries, in_bytes (file bytes), out_bytes
     (member bodies), zip_bytes, kernel_ms (deflate + CRC-32 kernels, CUDA events), n_chunks, n_stored_chunks,
-    n_fixed_chunks and the copy times.  ctx=None: the context the strip path has already warmed up, if any, else a
-    new one on device LAMBDIPY_B200_DEVICE (default 0).  There is no CPU path: without a GPU this raises."""
+    n_fixed_chunks, n_opt_chunks and the copy times.  ctx=None: the context the strip path has already warmed up, if
+    any, else a new one on device LAMBDIPY_B200_DEVICE (default 0).  compresslevel: None keeps the default encoder,
+    9 selects the optimal parse (smaller, slower); anything else raises ValueError.  There is no CPU path: without a
+    GPU this raises."""
     from .tarball import _default_context
+    N.deflate_flags(compresslevel)
     own = False
     if ctx is None:
         ctx, own = _default_context()
     try:
-        with GpuZipEncoder(ctx, piece_bytes) as enc:
+        with GpuZipEncoder(ctx, piece_bytes, compresslevel=compresslevel) as enc:
             return write_zip(root_dir, zip_path, enc)
     finally:
         if own:

@@ -13,6 +13,11 @@ Trees: site-packages numpy + numpy.libs + scipy + scipy.libs, torch/lib, and a s
 * the card's name and power limit, read in the same run.
 
     python tools/measure_gzip.py [--out results/h100_gzip.jsonl] [--trees numpy_scipy,torch_lib,synthetic]
+                                 [--compresslevel 9]
+
+With --compresslevel 9 the GPU side is the thorough mode (LB2_DEFLATE_BEST) throughout, and each line also carries
+the default mode's size on the same stream, the zlib level-6 size, the greedy and the optimal-parse kernel times
+apart, and n_opt_chunks.
 
 One JSON line per tree is printed and appended to --out.
 """
@@ -74,12 +79,12 @@ def tar_stream(srcs):
     return buf.getvalue()
 
 
-def gpu_deflate(ctx, data, piece=64 << 20):
+def gpu_deflate(ctx, data, piece=64 << 20, flags=0):
     """the tar stream through lb2_gzip_* with two pieces in flight; returns (DEFLATE bytes, stats, wall s)"""
     import ctypes as C
     lib = ctx.lib
     g = C.c_void_p()
-    ctx.check(lib.lb2_gzip_create(ctx.h, 0, C.byref(g)))
+    ctx.check(lib.lb2_gzip_create(ctx.h, flags, C.byref(g)))
     bufs = [ctx.pinned_alloc(piece) for _ in range(2)]
     cap = N.gzip_bound(piece)
     out = ctx.pinned_alloc(cap)
@@ -113,10 +118,10 @@ def gpu_deflate(ctx, data, piece=64 << 20):
     return total, st.as_dict(), wall
 
 
-def measure(ctx, name, tmp, gpu):
+def measure(ctx, name, tmp, gpu, level=None):
     srcs = tree_sources(name, tmp)
     data = tar_stream(srcs)
-    body, st, wall = gpu_deflate(ctx, data)
+    body, st, wall = gpu_deflate(ctx, data, flags=N.deflate_flags(level))
     kernel_s = (st["deflate_ms"] + st["crc_ms"]) / 1e3
     t0 = time.perf_counter()
     lvl1 = len(zlib.compress(data, 1))
@@ -124,7 +129,7 @@ def measure(ctx, name, tmp, gpu):
 
     gpu_path, ref_path = os.path.join(tmp, name + ".gpu.tar.gz"), os.path.join(tmp, name + ".ref.tar.gz")
     t0 = time.perf_counter()
-    tarball.gzip_tarball(srcs, gpu_path, ctx=ctx)
+    tarball.gzip_tarball(srcs, gpu_path, ctx=ctx, compresslevel=level)
     gpu_e2e = time.perf_counter() - t0
     t0 = time.perf_counter()
     with tarfile.open(ref_path, "w:gz") as tar:
@@ -137,7 +142,7 @@ def measure(ctx, name, tmp, gpu):
     gpu_file, ref_file = os.path.getsize(gpu_path), os.path.getsize(ref_path)
     os.remove(gpu_path)
     os.remove(ref_path)
-    return {
+    rec = {
         "tree": name, "sources": [os.path.relpath(p, SITE) if p.startswith(SITE) else os.path.basename(p) for p in srcs],
         "tar_bytes": len(data), "gpu": gpu,
         "deflate_kernel_ms": round(st["deflate_ms"], 3), "crc_kernel_ms": round(st["crc_ms"], 3),
@@ -151,12 +156,26 @@ def measure(ctx, name, tmp, gpu):
         "e2e_speedup": round(ref_e2e / gpu_e2e, 2), "gpu_file_bytes": gpu_file, "ref_file_bytes": ref_file,
         "tar_streams_equal": same,
     }
+    if level is not None:
+        default_body, dst, _ = gpu_deflate(ctx, data)
+        t0 = time.perf_counter()
+        lvl6 = len(zlib.compress(data, 6))
+        rec.update({
+            "compresslevel": level, "n_opt_chunks": st["n_opt_chunks"],
+            "greedy_kernel_ms": round(st["deflate_ms"] - st["best_ms"], 3), "best_kernel_ms": round(st["best_ms"], 3),
+            "best_kernel_GBps": round(len(data) / (st["best_ms"] / 1e3) / 1e9, 3) if st["best_ms"] else None,
+            "deflate_bytes_best": body, "deflate_bytes_default": default_body, "ratio_default": round(default_body / len(data), 4),
+            "ratio_zlib6": round(lvl6 / len(data), 4), "zlib6_s": round(time.perf_counter() - t0, 3),
+            "default_deflate_kernel_ms": round(dst["deflate_ms"], 3),
+        })
+    return rec
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=os.path.join(ROOT, "results", "h100_gzip.jsonl"))
     ap.add_argument("--trees", default="numpy_scipy,torch_lib,synthetic")
+    ap.add_argument("--compresslevel", type=int, default=None, choices=[9])
     args = ap.parse_args()
     gpu = gpu_info()
     with N.Context(0) as ctx:
@@ -164,7 +183,7 @@ def main():
         tmp = tempfile.mkdtemp(prefix="lb2_gzip_")
         try:
             for name in args.trees.split(","):
-                rec = measure(ctx, name, tmp, gpu)
+                rec = measure(ctx, name, tmp, gpu, args.compresslevel)
                 line = json.dumps(rec)
                 print(line, flush=True)
                 os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)

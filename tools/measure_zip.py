@@ -15,6 +15,10 @@ of BASELINE config 2, and a seeded synthetic tree of many small files (Python-li
 * the card's name and power limit, read in the same run.
 
     python tools/measure_zip.py [--out results/h100_zip.jsonl] [--trees numpy_scipy,config2,small_files] [--reps 3]
+                                [--compresslevel 9]
+
+With --compresslevel 9 zip_tree runs in the thorough mode (LB2_DEFLATE_BEST), and each line also carries the default
+mode's zip size, a zlib level-9 zip's, the greedy and the optimal-parse kernel times apart, and n_opt_chunks.
 
 One JSON line per tree is printed and appended to --out.
 """
@@ -80,10 +84,24 @@ def best(fn, reps):
     return t, r
 
 
-def measure(ctx, name, tmp, gpu, reps):
+def zlib_zip(root, path, level):
+    with zipfile.ZipFile(path, "w", compression=zipfile.ZIP_DEFLATED, compresslevel=level) as zf:
+        for p, zi in zipfile_gpu.tree_entries(root):
+            zf.write(p, zi.filename)
+    n = os.path.getsize(path)
+    os.remove(path)
+    return n
+
+
+def measure(ctx, name, tmp, gpu, reps, level=None):
     root = make_tree(name, tmp)
     gpu_path, ref_path, z1_path = (os.path.join(tmp, name + s) for s in (".gpu.zip", ".ref", ".z1.zip"))
-    gpu_s, st = best(lambda: zipfile_gpu.zip_tree(root, gpu_path, ctx=ctx), reps)
+    extra = {}
+    if level is not None:
+        dst = zipfile_gpu.zip_tree(root, gpu_path, ctx=ctx)
+        extra = {"zip_bytes_default": os.path.getsize(gpu_path), "default_deflate_kernel_ms": round(dst["deflate_ms"], 3),
+                 "zip_bytes_zlib9": zlib_zip(root, z1_path, 9)}
+    gpu_s, st = best(lambda: zipfile_gpu.zip_tree(root, gpu_path, ctx=ctx, compresslevel=level), reps)
     ref_s, _ = best(lambda: shutil.make_archive(ref_path, "zip", root), reps)
     with zipfile.ZipFile(z1_path, "w", compression=zipfile.ZIP_DEFLATED, compresslevel=1) as zf:
         for path, zi in zipfile_gpu.tree_entries(root):
@@ -96,7 +114,11 @@ def measure(ctx, name, tmp, gpu, reps):
     for p in (gpu_path, ref_path + ".zip", z1_path):
         os.remove(p)
     kernel_s = st["kernel_ms"] / 1e3
-    return {
+    if level is not None:
+        extra.update({"compresslevel": level, "n_opt_chunks": st["n_opt_chunks"],
+                      "greedy_kernel_ms": round(st["deflate_ms"] - st["best_ms"], 3), "best_kernel_ms": round(st["best_ms"], 3),
+                      "best_kernel_GBps": round(st["in_bytes"] / (st["best_ms"] / 1e3) / 1e9, 3) if st["best_ms"] else None})
+    return extra | {
         "tree": name, "gpu": gpu, "files": st["files"], "entries": st["entries"], "in_bytes": st["in_bytes"],
         "n_chunks": st["n_chunks"], "n_stored_chunks": st["n_stored_chunks"], "n_fixed_chunks": st["n_fixed_chunks"],
         "deflate_kernel_ms": round(st["deflate_ms"], 3), "crc_kernel_ms": round(st["crc_ms"], 3),
@@ -114,6 +136,7 @@ def main():
     ap.add_argument("--out", default=os.path.join(ROOT, "results", "h100_zip.jsonl"))
     ap.add_argument("--trees", default="numpy_scipy,config2,small_files")
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--compresslevel", type=int, default=None, choices=[9])
     args = ap.parse_args()
     gpu = gpu_info()
     with N.Context(0) as ctx:
@@ -125,7 +148,7 @@ def main():
                 f.write(os.urandom(1 << 20) + bytes(1 << 20))
             zipfile_gpu.zip_tree(warm, os.path.join(tmp, "warm.zip"), ctx=ctx)   # module load, first allocations
             for name in args.trees.split(","):
-                line = json.dumps(measure(ctx, name, tmp, gpu, args.reps))
+                line = json.dumps(measure(ctx, name, tmp, gpu, args.reps, args.compresslevel))
                 print(line, flush=True)
                 os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
                 with open(args.out, "a") as f:
