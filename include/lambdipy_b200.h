@@ -332,6 +332,60 @@ int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_
 int lb2_inflate_read(lb2_inflate *d, void *h_out, uint64_t cap);
 void lb2_inflate_destroy(lb2_inflate *d);
 
+/* ---- zip reader: every member of a zip decoded and checked on the GPU in one batch ------------------ */
+/* What `ZipFile.extractall` and `ZipFile.testzip` spend their time on.  The caller parses the zip (central directory
+ * and local headers) and uploads a buffer holding the member bodies; the library decodes every member and computes
+ * its CRC-32 on the device.  Each member is its own raw DEFLATE stream (method 8) or stored as it is (method 0).
+ *
+ * members[i] names the body h_in[body_off .. body_off + body_len) and the size and CRC-32 the archive records for
+ * it.  Member i's output is placed at results[i].out_off: the exclusive scan of the sizes, each rounded up to 16
+ * bytes.  Every bit a decoder reads is bounded by the member's own body.  A DEFLATE body of at most one span
+ * (LB2_INFLATE_SPAN_KB, read at each call, default 128) is decoded whole by one thread straight into its output; a
+ * larger one runs the speculative span pipeline of lb2_inflate_run, its spans batched with every other member's in
+ * each launch.  STORED bodies are copied on the device.
+ *
+ * results[i].status is the member's own: LB2_UNZIP_OK, LB2_UNZIP_BAD_DATA (invalid or truncated DEFLATE),
+ * LB2_UNZIP_WRONG_SIZE (more or fewer bytes than out size; a STORED body whose length is not its size) or
+ * LB2_UNZIP_BAD_CRC (results[i].crc32, computed on the device, differs from the member's crc32).  A bad member never
+ * changes another member's bytes or status, and the run itself still returns LB2_OK.
+ *
+ * Everything in the table is checked before any launch: a method other than 0 or 8, a body outside [0, n) or output
+ * sizes that overflow give LB2_E_ARG; a batch that does not fit in device memory (about n + 3 bytes per output byte
+ * when a member takes the span pipeline, n + 1 otherwise) gives LB2_E_CAPACITY.  The decoded bytes stay on the device
+ * until lb2_unzip_read copies them out (the next run replaces them).  Destroy the reader before its context. */
+typedef struct lb2_unzip lb2_unzip;
+typedef struct lb2_unzip_member {
+  uint64_t body_off, body_len;    /* the member's body in h_in                                                   */
+  uint64_t size;                  /* uncompressed size, from the central directory                               */
+  uint32_t crc32;                 /* CRC-32, from the central directory                                          */
+  uint32_t method;                /* 0 (stored) or 8 (DEFLATE)                                                   */
+} lb2_unzip_member;
+#define LB2_UNZIP_OK 0
+#define LB2_UNZIP_BAD_DATA 1
+#define LB2_UNZIP_WRONG_SIZE 2
+#define LB2_UNZIP_BAD_CRC 3
+typedef struct lb2_unzip_result {
+  uint64_t out_off;               /* the member's bytes in the lb2_unzip_read buffer                             */
+  uint32_t crc32;                 /* CRC-32 of those bytes (meaningful when the status is OK or BAD_CRC)         */
+  int32_t status;                 /* LB2_UNZIP_*                                                                 */
+} lb2_unzip_result;
+typedef struct lb2_unzip_stats {
+  uint64_t in_bytes, out_bytes;   /* buffer bytes uploaded, sum of the member sizes                              */
+  uint32_t n_members, n_stored, n_small, n_large;  /* members in all and on each path (copy, one span, pipeline) */
+  uint32_t n_spans;               /* spans the larger members were decoded in                                    */
+  uint32_t n_rounds;              /* count rounds (every chain advances in each)                                 */
+  uint32_t n_rejected, n_absorbed; /* as in lb2_inflate_stats, summed over the members                           */
+  uint32_t n_bad;                 /* members whose status is not LB2_UNZIP_OK                                    */
+  float h2d_ms, copy_ms, small_ms, find_ms, count_ms, decode_ms, resolve_ms, crc_ms;  /* CUDA events             */
+} lb2_unzip_stats;
+int lb2_unzip_create(lb2_ctx *ctx, uint32_t flags /* 0 */, lb2_unzip **u);
+/* decode members[0 .. n_members) of the buffer h_in (n bytes); *out_n = bytes lb2_unzip_read copies out */
+int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_member *members, uint32_t n_members,
+                  uint64_t *out_n, lb2_unzip_result *results, lb2_unzip_stats *stats);
+/* copy the output of the last successful run to h_out (cap >= *out_n) */
+int lb2_unzip_read(lb2_unzip *u, void *h_out, uint64_t cap);
+void lb2_unzip_destroy(lb2_unzip *u);
+
 #ifdef __cplusplus
 }
 #endif

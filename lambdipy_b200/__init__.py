@@ -11,6 +11,8 @@ Public surface:
     tarball.prepare_tarfile                     mirror of the reference's prepare_tarfile
     zip_tree(root_dir, zip_path)                the Lambda deployment zip of a tree (shutil.make_archive's
                                                 archive), every member's DEFLATE body compressed on the GPU
+    extract_zip(zip_path, directory)            ZipFile.extractall's tree, every member inflated on the GPU
+    testzip(zip_path)                           ZipFile.testzip's answer, every member checked on the GPU
     patch.apply()                               monkey-patch an installed lambdipy in place
 The byte work is done by liblambdipy_b200.so (CUDA, C ABI in include/lambdipy_b200.h).
 """
@@ -24,7 +26,7 @@ def __getattr__(name):
     if name in ("gzip_tarball", "gunzip"):
         from . import tarball
         return getattr(tarball, name)
-    if name == "zip_tree":
+    if name in ("zip_tree", "extract_zip", "testzip"):
         from . import zipfile_gpu
-        return zipfile_gpu.zip_tree
+        return getattr(zipfile_gpu, name)
     raise AttributeError(name)

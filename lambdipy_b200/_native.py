@@ -27,6 +27,7 @@ EXPORTS = [
     "lb2_gzip_create", "lb2_gzip_submit", "lb2_gzip_collect", "lb2_gzip_finish", "lb2_gzip_destroy",
     "lb2_inflate_create", "lb2_inflate_run", "lb2_inflate_read", "lb2_inflate_destroy",
     "lb2_zip_create", "lb2_zip_submit", "lb2_zip_collect", "lb2_zip_destroy",
+    "lb2_unzip_create", "lb2_unzip_run", "lb2_unzip_read", "lb2_unzip_destroy",
 ]
 ZIP_CONTINUES, ZIP_MORE = 1, 2
 DEFLATE_BEST = 1  # LB2_DEFLATE_BEST
@@ -102,6 +103,28 @@ class InflateStats(C.Structure):
         ("n_rounds", C.c_uint32), ("n_rejected", C.c_uint32), ("n_absorbed", C.c_uint32),
         ("find_ms", C.c_float), ("count_ms", C.c_float), ("decode_ms", C.c_float), ("resolve_ms", C.c_float),
         ("crc_ms", C.c_float), ("h2d_ms", C.c_float),
+    ]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class UnzipMember(C.Structure):
+    _fields_ = [("body_off", C.c_uint64), ("body_len", C.c_uint64), ("size", C.c_uint64), ("crc32", C.c_uint32),
+                ("method", C.c_uint32)]
+
+
+class UnzipResult(C.Structure):
+    _fields_ = [("out_off", C.c_uint64), ("crc32", C.c_uint32), ("status", C.c_int32)]
+
+
+class UnzipStats(C.Structure):
+    _fields_ = [
+        ("in_bytes", C.c_uint64), ("out_bytes", C.c_uint64), ("n_members", C.c_uint32), ("n_stored", C.c_uint32),
+        ("n_small", C.c_uint32), ("n_large", C.c_uint32), ("n_spans", C.c_uint32), ("n_rounds", C.c_uint32),
+        ("n_rejected", C.c_uint32), ("n_absorbed", C.c_uint32), ("n_bad", C.c_uint32),
+        ("h2d_ms", C.c_float), ("copy_ms", C.c_float), ("small_ms", C.c_float), ("find_ms", C.c_float),
+        ("count_ms", C.c_float), ("decode_ms", C.c_float), ("resolve_ms", C.c_float), ("crc_ms", C.c_float),
     ]
 
     def as_dict(self):
@@ -208,6 +231,15 @@ def load():
     lib.lb2_zip_collect.restype = C.c_int
     lib.lb2_zip_destroy.argtypes = [vp]
     lib.lb2_zip_destroy.restype = None
+    lib.lb2_unzip_create.argtypes = [vp, C.c_uint32, C.POINTER(vp)]
+    lib.lb2_unzip_create.restype = C.c_int
+    lib.lb2_unzip_run.argtypes = [vp, vp, C.c_uint64, C.POINTER(UnzipMember), C.c_uint32, u64p, C.POINTER(UnzipResult),
+                                  C.POINTER(UnzipStats)]
+    lib.lb2_unzip_run.restype = C.c_int
+    lib.lb2_unzip_read.argtypes = [vp, vp, C.c_uint64]
+    lib.lb2_unzip_read.restype = C.c_int
+    lib.lb2_unzip_destroy.argtypes = [vp]
+    lib.lb2_unzip_destroy.restype = None
     _lib = lib
     return lib
 

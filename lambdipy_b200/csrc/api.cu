@@ -830,27 +830,40 @@ struct lb2_inflate {
   uint8_t *d_in = nullptr, *d_out = nullptr;
   uint16_t *d_arena = nullptr;
   uint64_t *d_cand = nullptr;
+  ifl::FindJob *d_find = nullptr;
   ifl::SpanJob *d_jobs = nullptr;
   ifl::SpanResult *d_res = nullptr;
-  uint32_t *d_chunk_crc = nullptr, *d_crc = nullptr;
+  uint32_t *d_chunk_crc = nullptr, *d_crc = nullptr, *d_first = nullptr;
   int32_t *d_err = nullptr;
-  uint64_t cap_in = 0, cap_cand = 0, cap_jobs = 0, cap_res = 0, cap_arena = 0, cap_out = 0, cap_chunks = 0;
+  uint64_t cap_in = 0, cap_cand = 0, cap_find = 0, cap_jobs = 0, cap_res = 0, cap_arena = 0, cap_out = 0, cap_chunks = 0;
   cudaEvent_t ev[2] = {nullptr, nullptr};
   uint64_t out_n = 0;
   bool have = false;
 };
 
 // (re)allocates *p for `need` elements when `cap` is smaller; LB2_E_CAPACITY when the device has no room
-template <class T> static int ifl_grow(lb2_ctx *ctx, T **p, uint64_t &cap, uint64_t need) {
+template <class T> static int ifl_grow(lb2_ctx *ctx, T **p, uint64_t &cap, uint64_t need,
+                                       const char *what = "lb2_inflate_run: the stream") {
   if (need <= cap) return LB2_OK;
   const cudaError_t e = regrow(p, cap, need, 16);
   if (e == cudaErrorMemoryAllocation) {
     cudaGetLastError();
-    ctx->err = "lb2_inflate_run: the stream does not fit in device memory";
+    ctx->err = std::string(what) + " does not fit in device memory";
     return LB2_E_CAPACITY;
   }
   CK(e);
   return LB2_OK;
+}
+
+// LB2_INFLATE_SPAN_KB (default 128): the nominal span, read at each run
+static bool ifl_span(lb2_ctx *ctx, uint64_t &span) {
+  span = 128 << 10;
+  if (const char *v = getenv("LB2_INFLATE_SPAN_KB")) {
+    const long kb = atol(v);
+    if (kb < 1) { ctx->err = "LB2_INFLATE_SPAN_KB must be a positive number of KB"; return false; }
+    span = (uint64_t)kb << 10;
+  }
+  return true;
 }
 
 static float ifl_elapsed(lb2_inflate *d) {
@@ -871,7 +884,8 @@ int lb2_inflate_create(lb2_ctx *ctx, uint32_t flags, lb2_inflate **out) {
   cudaError_t e;
   if ((e = cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking)) != cudaSuccess ||
       (e = cudaEventCreate(&d->ev[0])) != cudaSuccess || (e = cudaEventCreate(&d->ev[1])) != cudaSuccess ||
-      (e = cudaMalloc(&d->d_crc, sizeof(uint32_t))) != cudaSuccess || (e = cudaMalloc(&d->d_err, sizeof(int32_t))) != cudaSuccess) {
+      (e = cudaMalloc(&d->d_crc, sizeof(uint32_t))) != cudaSuccess || (e = cudaMalloc(&d->d_err, sizeof(int32_t))) != cudaSuccess ||
+      (e = cudaMalloc(&d->d_first, 2 * sizeof(uint32_t))) != cudaSuccess) {
     ctx->err = std::string("lb2_inflate_create: ") + cudaGetErrorString(e);
     lb2_inflate_destroy(d);
     return LB2_E_CUDA;
@@ -885,7 +899,7 @@ void lb2_inflate_destroy(lb2_inflate *d) {
   cudaSetDevice(d->ctx->device);
   if (d->stream) cudaStreamSynchronize(d->stream);
   cudaFree(d->d_in); cudaFree(d->d_out); cudaFree(d->d_arena); cudaFree(d->d_cand); cudaFree(d->d_jobs); cudaFree(d->d_res);
-  cudaFree(d->d_chunk_crc); cudaFree(d->d_crc); cudaFree(d->d_err);
+  cudaFree(d->d_chunk_crc); cudaFree(d->d_crc); cudaFree(d->d_err); cudaFree(d->d_find); cudaFree(d->d_first);
   for (auto &e : d->ev) if (e) cudaEventDestroy(e);
   if (d->stream) cudaStreamDestroy(d->stream);
   delete d;
@@ -899,18 +913,18 @@ int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_
   d->have = false;
   *out_n = 0;
   lb2_inflate_stats st{};
-  uint64_t span = 128 << 10;
-  if (const char *v = getenv("LB2_INFLATE_SPAN_KB")) {
-    const long kb = atol(v);
-    if (kb < 1) { ctx->err = "LB2_INFLATE_SPAN_KB must be a positive number of KB"; return LB2_E_ARG; }
-    span = (uint64_t)kb << 10;
-  }
+  uint64_t span;
+  if (!ifl_span(ctx, span)) return LB2_E_ARG;
   const uint32_t n_spans = n > span ? (uint32_t)((n + span - 1) / span) : 1;
   cudaStream_t s = d->stream;
   int rc;
   if ((rc = ifl_grow(ctx, &d->d_in, d->cap_in, n)) || (rc = ifl_grow(ctx, &d->d_cand, d->cap_cand, n_spans)) ||
-      (rc = ifl_grow(ctx, &d->d_jobs, d->cap_jobs, n_spans)) || (rc = ifl_grow(ctx, &d->d_res, d->cap_res, n_spans)))
+      (rc = ifl_grow(ctx, &d->d_jobs, d->cap_jobs, n_spans)) || (rc = ifl_grow(ctx, &d->d_res, d->cap_res, n_spans)) ||
+      (rc = ifl_grow(ctx, &d->d_find, d->cap_find, n_spans)))
     return rc;
+  std::vector<ifl::FindJob> find;  // the one stream's nominal spans k >= 1
+  for (uint32_t k = 1; k < n_spans; k++) find.push_back(ifl::FindJob{0, n, k, 0});
+  if (!find.empty()) CK(cudaMemcpyAsync(d->d_find, find.data(), find.size() * sizeof(ifl::FindJob), cudaMemcpyHostToDevice, d->stream));
   // upload
   CK(cudaEventRecord(d->ev[0], s));
   if (n) CK(cudaMemcpyAsync(d->d_in, h_in, n, cudaMemcpyHostToDevice, s));
@@ -920,10 +934,10 @@ int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_
   // candidates
   std::vector<uint64_t> cand(n_spans, ifl::KEY_NONE);
   CK(cudaEventRecord(d->ev[0], s));
-  launch_inflate_find(d->d_in, n, span, n_spans, d->d_cand, s);
+  launch_inflate_find(d->d_in, span, d->d_find, (uint32_t)find.size(), d->d_cand, s);
   CK(cudaGetLastError());
   CK(cudaEventRecord(d->ev[1], s));
-  if (n_spans > 1) CK(cudaMemcpyAsync(cand.data() + 1, d->d_cand + 1, (n_spans - 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+  if (n_spans > 1) CK(cudaMemcpyAsync(cand.data() + 1, d->d_cand, (n_spans - 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   st.find_ms = ifl_elapsed(d);
   // count rounds and chain
@@ -938,7 +952,7 @@ int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_
     for (size_t i = 0; i < p.size(); i++) jobs[i] = c.job[p[i]];
     CK(cudaMemcpyAsync(d->d_jobs, jobs.data(), jobs.size() * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
     CK(cudaEventRecord(d->ev[0], s));
-    launch_inflate_count(d->d_in, n, d->d_jobs, (uint32_t)jobs.size(), d->d_res, s);
+    launch_inflate_count(d->d_in, d->d_jobs, (uint32_t)jobs.size(), d->d_res, s);
     CK(cudaGetLastError());
     CK(cudaEventRecord(d->ev[1], s));
     CK(cudaMemcpyAsync(res.data(), d->d_res, res.size() * sizeof(ifl::SpanResult), cudaMemcpyDeviceToHost, s));
@@ -968,13 +982,15 @@ int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_
   CK(cudaMemcpyAsync(d->d_jobs, c.job.data(), n_used * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
   CK(cudaMemsetAsync(d->d_err, 0, sizeof(int32_t), s));
   CK(cudaEventRecord(d->ev[0], s));
-  launch_inflate_decode(d->d_in, n, d->d_jobs, n_used, d->d_arena, d->d_err, s);
+  launch_inflate_decode(d->d_in, d->d_jobs, n_used, d->d_arena, d->d_err, s);
   CK(cudaGetLastError());
   CK(cudaEventRecord(d->ev[1], s));
   CK(cudaEventSynchronize(d->ev[1]));
   st.decode_ms = ifl_elapsed(d);
   CK(cudaEventRecord(d->ev[0], s));
-  launch_inflate_resolve(d->d_arena, d->d_out, d->d_jobs, n_used, d->d_err, s);
+  const uint32_t span_range[2] = {0, n_used};
+  CK(cudaMemcpyAsync(d->d_first, span_range, sizeof span_range, cudaMemcpyHostToDevice, s));
+  launch_inflate_resolve(d->d_arena, d->d_out, d->d_jobs, n_used, d->d_first, 1, d->d_err, s);
   CK(cudaGetLastError());
   CK(cudaEventRecord(d->ev[1], s));
   CK(cudaEventSynchronize(d->ev[1]));
@@ -1007,6 +1023,268 @@ int lb2_inflate_read(lb2_inflate *d, void *h_out, uint64_t cap) {
   if (!h_out && d->out_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
   CK(cudaSetDevice(ctx->device));
   if (d->out_n) CK(cudaMemcpy(h_out, d->d_out, d->out_n, cudaMemcpyDeviceToHost));
+  return LB2_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------- zip reader
+// The inflate pipeline over a member table (ifl::Batch in inflate_core.cuh).  The archive bytes are uploaded once;
+// STORED members are copied, one-span members decoded whole, larger ones run find / count rounds / decode / resolve
+// with every member's spans in the same launches; then the writer's CRC and scan kernels give each member's CRC-32.
+static_assert(sizeof(ifl::Member) == 40 && sizeof(lb2_unzip_member) == 32, "member table entries");
+
+struct lb2_unzip {
+  lb2_ctx *ctx = nullptr;
+  cudaStream_t stream = nullptr;
+  uint8_t *d_in = nullptr, *d_out = nullptr, *d_tab = nullptr;
+  uint16_t *d_arena = nullptr;
+  uint64_t *d_cand = nullptr, *d_chunk_off = nullptr;
+  ifl::FindJob *d_find = nullptr;
+  ifl::SpanJob *d_jobs = nullptr, *d_small = nullptr;
+  ifl::SpanResult *d_res = nullptr;
+  ifl::Member *d_members = nullptr;
+  uint32_t *d_idx = nullptr, *d_first = nullptr, *d_chunk_crc = nullptr, *d_zero = nullptr;
+  int32_t *d_status = nullptr;
+  GzSegResult *d_seg = nullptr;
+  GzResult *d_gres = nullptr;
+  uint64_t cap_in = 0, cap_out = 0, cap_tab = 0, cap_arena = 0, cap_cand = 0, cap_chunk_off = 0, cap_find = 0, cap_jobs = 0,
+           cap_small = 0, cap_res = 0, cap_members = 0, cap_idx = 0, cap_first = 0, cap_chunk_crc = 0, cap_zero = 0,
+           cap_status = 0, cap_seg = 0, cap_gres = 0;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  uint64_t out_n = 0;
+  bool have = false;
+};
+
+static float uz_elapsed(lb2_unzip *u) {
+  float ms = 0;
+  cudaEventElapsedTime(&ms, u->ev[0], u->ev[1]);
+  return ms;
+}
+
+extern "C" {
+
+int lb2_unzip_create(lb2_ctx *ctx, uint32_t flags, lb2_unzip **out) {
+  if (!ctx || !out) { if (ctx) ctx->err = "NULL argument"; return LB2_E_ARG; }
+  *out = nullptr;
+  if (flags) { ctx->err = "lb2_unzip_create: no flags are defined"; return LB2_E_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  lb2_unzip *u = new lb2_unzip();
+  u->ctx = ctx;
+  cudaError_t e;
+  if ((e = cudaStreamCreateWithFlags(&u->stream, cudaStreamNonBlocking)) != cudaSuccess ||
+      (e = cudaEventCreate(&u->ev[0])) != cudaSuccess || (e = cudaEventCreate(&u->ev[1])) != cudaSuccess) {
+    ctx->err = std::string("lb2_unzip_create: ") + cudaGetErrorString(e);
+    lb2_unzip_destroy(u);
+    return LB2_E_CUDA;
+  }
+  *out = u;
+  return LB2_OK;
+}
+
+void lb2_unzip_destroy(lb2_unzip *u) {
+  if (!u) return;
+  cudaSetDevice(u->ctx->device);
+  if (u->stream) cudaStreamSynchronize(u->stream);
+  cudaFree(u->d_in); cudaFree(u->d_out); cudaFree(u->d_tab); cudaFree(u->d_arena); cudaFree(u->d_cand);
+  cudaFree(u->d_chunk_off); cudaFree(u->d_find); cudaFree(u->d_jobs); cudaFree(u->d_small); cudaFree(u->d_res);
+  cudaFree(u->d_members); cudaFree(u->d_idx); cudaFree(u->d_first); cudaFree(u->d_chunk_crc); cudaFree(u->d_zero);
+  cudaFree(u->d_status); cudaFree(u->d_seg); cudaFree(u->d_gres);
+  for (auto &e : u->ev) if (e) cudaEventDestroy(e);
+  if (u->stream) cudaStreamDestroy(u->stream);
+  delete u;
+}
+
+int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_member *members, uint32_t n_members,
+                  uint64_t *out_n, lb2_unzip_result *results, lb2_unzip_stats *stats) {
+  if (!u) return LB2_E_ARG;
+  lb2_ctx *ctx = u->ctx;
+  if ((!h_in && n) || !out_n || (n_members && (!members || !results))) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  u->have = false;
+  *out_n = 0;
+  // everything the archive says is checked before any launch
+  std::vector<ifl::Member> m(n_members);
+  uint64_t total = 0, n_chunks = 0;
+  for (uint32_t i = 0; i < n_members; i++) {
+    const lb2_unzip_member &x = members[i];
+    const std::string which = "lb2_unzip_run: member " + std::to_string(i);
+    if (x.method != 0 && x.method != 8) { ctx->err = which + ": method " + std::to_string(x.method) + " is not 0 or 8"; return LB2_E_ARG; }
+    if (x.body_off > n || x.body_len > n - x.body_off) { ctx->err = which + ": body outside the buffer"; return LB2_E_ARG; }
+    if (x.size > UINT64_MAX - 32 - total) { ctx->err = which + ": output size overflows"; return LB2_E_ARG; }
+    m[i] = ifl::Member{x.body_off, x.body_len, total, x.size, x.crc32, x.method};
+    total = (total + x.size + 15) & ~15ull;  // 16-byte-aligned output offsets (the CRC kernel's vector loads)
+    n_chunks += x.size ? (x.size + GZ_CHUNK - 1) / GZ_CHUNK : 1;
+  }
+  if (n_chunks > UINT32_MAX / 2) { ctx->err = "lb2_unzip_run: too many output chunks"; return LB2_E_ARG; }
+  uint64_t span;
+  if (!ifl_span(ctx, span)) return LB2_E_ARG;
+  CK(cudaSetDevice(ctx->device));
+  lb2_unzip_stats st{};
+  st.n_members = n_members;
+  st.in_bytes = n;
+  ifl::Batch b;
+  b.init(m.data(), n_members, span);
+  st.n_stored = (uint32_t)b.stored.size();
+  st.n_small = (uint32_t)b.small.size();
+  st.n_large = (uint32_t)b.large.size();
+  const char *what = "lb2_unzip_run: the archive";
+  const uint64_t tab = n_chunks * sizeof(GzChunk) + (uint64_t)n_members * sizeof(GzSeg);
+  int rc;
+  if ((rc = ifl_grow(ctx, &u->d_in, u->cap_in, n, what)) || (rc = ifl_grow(ctx, &u->d_out, u->cap_out, total, what)) ||
+      (rc = ifl_grow(ctx, &u->d_members, u->cap_members, n_members, what)) ||
+      (rc = ifl_grow(ctx, &u->d_status, u->cap_status, n_members, what)) ||
+      (rc = ifl_grow(ctx, &u->d_idx, u->cap_idx, b.stored.size(), what)) ||
+      (rc = ifl_grow(ctx, &u->d_small, u->cap_small, b.small.size(), what)) ||
+      (rc = ifl_grow(ctx, &u->d_find, u->cap_find, b.find.size(), what)) ||
+      (rc = ifl_grow(ctx, &u->d_cand, u->cap_cand, b.find.size(), what)) ||
+      (rc = ifl_grow(ctx, &u->d_tab, u->cap_tab, tab, what)) ||
+      (rc = ifl_grow(ctx, &u->d_chunk_crc, u->cap_chunk_crc, n_chunks, what)) ||
+      (rc = ifl_grow(ctx, &u->d_zero, u->cap_zero, 2 * n_chunks + 1, what)) ||
+      (rc = ifl_grow(ctx, &u->d_chunk_off, u->cap_chunk_off, n_chunks, what)) ||
+      (rc = ifl_grow(ctx, &u->d_seg, u->cap_seg, n_members, what)) || (rc = ifl_grow(ctx, &u->d_gres, u->cap_gres, 1, what)))
+    return rc;
+  cudaStream_t s = u->stream;
+  // upload: the archive, the member table and the host-known statuses
+  CK(cudaEventRecord(u->ev[0], s));
+  if (n) CK(cudaMemcpyAsync(u->d_in, h_in, n, cudaMemcpyHostToDevice, s));
+  CK(cudaEventRecord(u->ev[1], s));
+  if (n_members) {
+    CK(cudaMemcpyAsync(u->d_members, m.data(), n_members * sizeof(ifl::Member), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(u->d_status, b.status.data(), n_members * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  }
+  if (!b.stored.empty()) CK(cudaMemcpyAsync(u->d_idx, b.stored.data(), b.stored.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+  if (!b.small.empty()) CK(cudaMemcpyAsync(u->d_small, b.small.data(), b.small.size() * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
+  if (!b.find.empty()) CK(cudaMemcpyAsync(u->d_find, b.find.data(), b.find.size() * sizeof(ifl::FindJob), cudaMemcpyHostToDevice, s));
+  CK(cudaStreamSynchronize(s));
+  st.h2d_ms = uz_elapsed(u);
+  // STORED members, then the one-span members
+  CK(cudaEventRecord(u->ev[0], s));
+  launch_unzip_copy(u->d_in, u->d_members, u->d_idx, (uint32_t)b.stored.size(), u->d_out, s);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(u->ev[1], s));
+  CK(cudaEventSynchronize(u->ev[1]));
+  st.copy_ms = uz_elapsed(u);
+  CK(cudaEventRecord(u->ev[0], s));
+  launch_unzip_small(u->d_in, u->d_small, (uint32_t)b.small.size(), u->d_out, u->d_status, s);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(u->ev[1], s));
+  CK(cudaEventSynchronize(u->ev[1]));
+  st.small_ms = uz_elapsed(u);
+  // larger members: candidates, then count rounds with one chain per member
+  if (!b.large.empty()) {
+    std::vector<uint64_t> cand(b.find.size());
+    CK(cudaEventRecord(u->ev[0], s));
+    launch_inflate_find(u->d_in, span, u->d_find, (uint32_t)b.find.size(), u->d_cand, s);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(u->ev[1], s));
+    if (!cand.empty()) CK(cudaMemcpyAsync(cand.data(), u->d_cand, cand.size() * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    st.find_ms = uz_elapsed(u);
+    b.start_chains(cand.data(), span);
+    std::vector<ifl::SpanJob> jobs;
+    std::vector<ifl::SpanResult> res;
+    std::vector<std::pair<uint32_t, uint32_t>> ref;
+    while (b.pending(jobs, ref)) {
+      if ((rc = ifl_grow(ctx, &u->d_jobs, u->cap_jobs, jobs.size(), what)) || (rc = ifl_grow(ctx, &u->d_res, u->cap_res, jobs.size(), what)))
+        return rc;
+      res.resize(jobs.size());
+      CK(cudaMemcpyAsync(u->d_jobs, jobs.data(), jobs.size() * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
+      CK(cudaEventRecord(u->ev[0], s));
+      launch_inflate_count(u->d_in, u->d_jobs, (uint32_t)jobs.size(), u->d_res, s);
+      CK(cudaGetLastError());
+      CK(cudaEventRecord(u->ev[1], s));
+      CK(cudaMemcpyAsync(res.data(), u->d_res, res.size() * sizeof(ifl::SpanResult), cudaMemcpyDeviceToHost, s));
+      CK(cudaStreamSynchronize(s));
+      st.count_ms += uz_elapsed(u);
+      b.set_results(ref, res.data());
+    }
+    st.n_rounds = b.n_rounds;
+    st.n_rejected = b.n_rejected();
+    st.n_absorbed = b.n_absorbed();
+    // decode the members whose chains ended at their recorded sizes into the u16 arena at their output offsets
+    std::vector<uint32_t> first;
+    b.layout(jobs, first);
+    st.n_spans = (uint32_t)jobs.size();
+    const uint32_t n_dec = (uint32_t)first.size() - 1;
+    if (n_dec) {
+      if ((rc = ifl_grow(ctx, &u->d_arena, u->cap_arena, total, what)) || (rc = ifl_grow(ctx, &u->d_jobs, u->cap_jobs, jobs.size(), what)) ||
+          (rc = ifl_grow(ctx, &u->d_first, u->cap_first, first.size(), what)))
+        return rc;
+      CK(cudaMemcpyAsync(u->d_jobs, jobs.data(), jobs.size() * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
+      CK(cudaMemcpyAsync(u->d_first, first.data(), first.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+      CK(cudaEventRecord(u->ev[0], s));
+      launch_inflate_decode(u->d_in, u->d_jobs, (uint32_t)jobs.size(), u->d_arena, u->d_status, s);
+      CK(cudaGetLastError());
+      CK(cudaEventRecord(u->ev[1], s));
+      CK(cudaEventSynchronize(u->ev[1]));
+      st.decode_ms = uz_elapsed(u);
+      CK(cudaEventRecord(u->ev[0], s));
+      launch_inflate_resolve(u->d_arena, u->d_out, u->d_jobs, (uint32_t)jobs.size(), u->d_first, n_dec, u->d_status, s);
+      CK(cudaGetLastError());
+      CK(cudaEventRecord(u->ev[1], s));
+      CK(cudaEventSynchronize(u->ev[1]));
+      st.resolve_ms = uz_elapsed(u);
+    }
+  }
+  // CRC-32 of every member: the writer's chunk table over the output, one segment per member
+  std::vector<GzSegResult> seg(n_members);
+  std::vector<int32_t> dev_status(n_members);
+  if (n_members) {
+    std::vector<uint8_t> h_tab(tab);
+    GzChunk *chunks = reinterpret_cast<GzChunk *>(h_tab.data());
+    GzSeg *segs = reinterpret_cast<GzSeg *>(h_tab.data() + n_chunks * sizeof(GzChunk));
+    uint32_t c = 0;
+    for (uint32_t i = 0; i < n_members; i++) {
+      segs[i] = GzSeg{m[i].out_off, m[i].out_len, c, GZ_SEG_ENDS};
+      uint64_t p = 0;
+      do {
+        const uint32_t len = (uint32_t)std::min<uint64_t>(GZ_CHUNK, m[i].out_len - p);
+        chunks[c++] = GzChunk{m[i].out_off + p, len, 0, i, 0};
+        p += len;
+      } while (p < m[i].out_len);
+    }
+    GzPieceArgs a{};
+    a.in = u->d_out; a.n = total; a.n_chunks = c; a.n_segs = n_members;
+    a.chunks = reinterpret_cast<const GzChunk *>(u->d_tab);
+    a.segs = reinterpret_cast<const GzSeg *>(u->d_tab + n_chunks * sizeof(GzChunk));
+    a.chunk_size = u->d_zero; a.chunk_mode = u->d_zero + n_chunks; a.crc_state = u->d_zero + 2 * n_chunks;
+    a.chunk_crc = u->d_chunk_crc; a.chunk_off = u->d_chunk_off; a.seg_res = u->d_seg; a.res = u->d_gres;
+    CK(cudaMemcpyAsync(u->d_tab, h_tab.data(), tab, cudaMemcpyHostToDevice, s));
+    CK(cudaMemsetAsync(u->d_zero, 0, (2 * n_chunks + 1) * sizeof(uint32_t), s));
+    CK(cudaEventRecord(u->ev[0], s));
+    launch_segment_crc32(a, s);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(u->ev[1], s));
+    CK(cudaMemcpyAsync(seg.data(), u->d_seg, n_members * sizeof(GzSegResult), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(dev_status.data(), u->d_status, n_members * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    st.crc_ms = uz_elapsed(u);
+  }
+  for (uint32_t i = 0; i < n_members; i++) {
+    // a status found on the host stands; a device one is the small kernel's, or a large member's span status (< 0)
+    int32_t r = b.status[i] != ifl::MS_OK ? b.status[i] : dev_status[i] < 0 ? (int32_t)ifl::MS_BAD_DATA : dev_status[i];
+    if (r == ifl::MS_OK && seg[i].crc32 != m[i].crc32) r = ifl::MS_BAD_CRC;
+    results[i].out_off = m[i].out_off;
+    results[i].crc32 = seg[i].crc32;
+    results[i].status = r;
+    st.n_bad += r != ifl::MS_OK;
+    st.out_bytes += m[i].out_len;
+  }
+  if (stats) *stats = st;
+  u->out_n = total;
+  u->have = true;
+  *out_n = total;
+  return LB2_OK;
+}
+
+int lb2_unzip_read(lb2_unzip *u, void *h_out, uint64_t cap) {
+  if (!u) return LB2_E_ARG;
+  lb2_ctx *ctx = u->ctx;
+  if (!u->have) { ctx->err = "lb2_unzip_read: no decoded batch (lb2_unzip_run failed or was not called)"; return LB2_E_STATE; }
+  if (cap < u->out_n) { ctx->err = "lb2_unzip_read: buffer smaller than the decoded batch"; return LB2_E_CAPACITY; }
+  if (!h_out && u->out_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  if (u->out_n) CK(cudaMemcpy(h_out, u->d_out, u->out_n, cudaMemcpyDeviceToHost));
   return LB2_OK;
 }
 

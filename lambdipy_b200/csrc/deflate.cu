@@ -947,6 +947,11 @@ void launch_crc32(const uint8_t *in, uint64_t n, uint32_t *chunk_crc, uint32_t *
   lb2_crc32_kernel<<<(unsigned)((n + GZ_CHUNK - 1) / GZ_CHUNK), CRC_THREADS, 0, s>>>(in, n, nullptr, chunk_crc);
   lb2_crc32_combine_kernel<<<1, SCAN_THREADS, 0, s>>>(chunk_crc, n, crc);
 }
+void launch_segment_crc32(const GzPieceArgs &a, cudaStream_t s) {
+  if (!a.n_segs) return;
+  lb2_crc32_kernel<<<a.n_chunks, CRC_THREADS, 0, s>>>(a.in, a.n, a.chunks, a.chunk_crc);
+  lb2_gzip_scan_kernel<<<1, SCAN_THREADS, 0, s>>>(a);
+}
 void launch_gzip_compact(const GzPieceArgs &a, cudaStream_t s) {
   lb2_gzip_scan_kernel<<<1, SCAN_THREADS, 0, s>>>(a);
   lb2_gzip_gather_kernel<<<(a.n_chunks + 7) / 8, 256, 0, s>>>(a);

@@ -14,6 +14,7 @@
 // (the header bits and padding in front of it may sit at several offsets, which all decode the same).
 #pragma once
 #include <cstdint>
+#include <utility>
 #include <vector>
 
 #ifdef __CUDACC__
@@ -304,6 +305,10 @@ struct SpanJob {
   uint64_t out_len;    // decode pass: the counted length
   uint32_t first;      // span 0: no window in front of it
   uint32_t pad;
+  // where the span's stream is: the kernels decode in[in_off .. in_off + in_n); out_base is the stream's first output
+  // byte in the arena (a window marker must not point before it); member indexes the per-stream status
+  uint64_t in_off, in_n, out_base;
+  uint32_t member, pad2;
 };
 struct SpanResult {
   uint64_t end_key;    // key where the span stopped (KEY_NONE after the final block)
@@ -327,9 +332,12 @@ IFL_HD void fixed_tables(DecodeState &st) {
 }
 
 // Decodes one span from job.start_key.  EMIT = false counts the output; EMIT = true writes it to out[0 .. job.out_len)
-// as u16: bytes, or 0x8000 | w for byte w of the 32 KB before the span.
-template <bool EMIT>
-IFL_HD void decode_span(const uint8_t *in, uint64_t n, const SpanJob &job, DecodeState &st, uint16_t *out,
+// as u16: bytes, or 0x8000 | w for byte w of the 32 KB before the span.  T = uint8_t is the byte-output variant for a
+// stream decoded whole by one decoder (job.first = 1: no window, so no markers); more or fewer bytes than job.out_len
+// give ST_OVERFLOW.
+template <class T> struct NoDeduce { typedef T type; };  // the output type is named, never deduced (out may be nullptr)
+template <bool EMIT, class T = uint16_t>
+IFL_HD void decode_span(const uint8_t *in, uint64_t n, const SpanJob &job, DecodeState &st, typename NoDeduce<T>::type *out,
                         SpanResult &res) {
   Bits b;
   const uint64_t start = key_bit(job.start_key);
@@ -414,7 +422,7 @@ IFL_HD void decode_span(const uint8_t *in, uint64_t n, const SpanJob &job, Decod
             uint32_t j = 0;
             for (uint32_t k = 0; k < len; k++) {  // repeats the last `dist` values when the match overlaps itself
               const int64_t s = src + j;
-              out[pos + k] = s < 0 ? (uint16_t)(0x8000u | (uint32_t)(32768 + s)) : out[s];
+              out[pos + k] = s < 0 ? (T)(0x8000u | (uint32_t)(32768 + s)) : out[s];
               if (++j == dist) j = 0;
             }
           }
@@ -438,11 +446,11 @@ IFL_HD void decode_span(const uint8_t *in, uint64_t n, const SpanJob &job, Decod
 }
 
 // ---- resolve: the value of output position i of a span whose output starts at `off` in the final arena -----------
-// Returns false for a window position before the stream start (corrupt data).
-IFL_HD bool resolve_value(uint16_t v, uint64_t off, const uint8_t *final_out, uint8_t &byte) {
+// Returns false for a window position before the stream start `base` (corrupt data).
+IFL_HD bool resolve_value(uint16_t v, uint64_t off, const uint8_t *final_out, uint8_t &byte, uint64_t base = 0) {
   if (!(v & 0x8000)) { byte = (uint8_t)v; return true; }
   const uint64_t w = v & 0x7FFF;
-  if (off + w < 32768) { byte = 0; return false; }
+  if (off + w < base + 32768) { byte = 0; return false; }
   byte = final_out[off + w - 32768];
   return true;
 }
@@ -463,8 +471,10 @@ struct Chain {
   bool done = false;
   int32_t error = ST_OK;
 
-  // cand[k]: the candidate key of nominal span k >= 1 (cand[0] is ignored); giveup: multiple of the span size
-  void init(const uint64_t *cand, uint32_t n_spans, uint64_t span_bytes, uint64_t n, uint32_t giveup) {
+  // cand[k]: the candidate key of nominal span k >= 1 (cand[0] is ignored); giveup: multiple of the span size;
+  // the stream is in[in_off .. in_off + n) of the kernels' input, `member` its index in a member table
+  void init(const uint64_t *cand, uint32_t n_spans, uint64_t span_bytes, uint64_t n, uint32_t giveup, uint64_t in_off = 0,
+            uint32_t member = 0) {
     n_bytes = n;
     n_nominal = n_spans;
     std::vector<uint64_t> nominal{0};
@@ -484,6 +494,11 @@ struct Chain {
       j.out_off = j.out_len = 0;
       j.first = i == 0;
       j.pad = 0;
+      j.in_off = in_off;
+      j.in_n = n;
+      j.out_base = 0;
+      j.member = member;
+      j.pad2 = 0;
     }
     res.assign(job.size(), SpanResult{});
     counted.assign(job.size(), 0);
@@ -543,19 +558,137 @@ struct Chain {
     }
     if (!done && !error && next == job.size()) error = ST_EOF;
   }
-  // after done: output offsets of the confirmed spans; returns the total output
-  uint64_t layout() {
+  // after done: output offsets of the confirmed spans, from `base` in the arena; returns the stream's total output
+  uint64_t layout(uint64_t base = 0) {
     uint64_t off = 0;
     for (size_t i = 0; i < job.size(); i++) {
-      job[i].out_off = off;
+      job[i].out_off = base + off;
       job[i].out_len = res[i].out_len;
       job[i].limit_bit = KEY_NONE;
+      job[i].out_base = base;
       off += res[i].out_len;
     }
     return off;
   }
   uint64_t in_bytes() const { return job.empty() ? 0 : (res.back().end_bit + 7) / 8; }
 };
+
+// ---- member table (host): many streams decoded in one batch (the zip reader) --------------------------------------
+// Each member is a raw DEFLATE (method 8) or STORED (method 0) body in[in_off .. in_off + in_len) whose output goes to
+// out[out_off .. out_off + out_len), out_len being the size the archive records.  A DEFLATE body of at most one span
+// is decoded whole by one thread (decode_span<true, uint8_t>, straight into the output); a larger one runs the
+// speculative pipeline above with a Chain of its own, its spans batched with those of the other members in every
+// launch.  Each member ends with one status; a bad member never touches another member's output or status.
+enum : int32_t { MS_OK = 0, MS_BAD_DATA = 1, MS_WRONG_SIZE = 2, MS_BAD_CRC = 3 };
+struct Member {
+  uint64_t in_off, in_len, out_off, out_len;
+  uint32_t crc32, method;
+};
+struct FindJob {  // nominal span k >= 1 of the stream in[in_off .. in_off + in_n)
+  uint64_t in_off, in_n;
+  uint32_t k, pad;
+};
+
+struct Batch {
+  std::vector<Member> m;
+  std::vector<int32_t> status;            // per member
+  std::vector<uint32_t> stored;           // members copied as they are
+  std::vector<SpanJob> small;             // one decode job per one-span member
+  std::vector<uint32_t> large;            // members run through the chain
+  std::vector<FindJob> find;              // their nominal spans k >= 1, member by member
+  std::vector<uint32_t> find_first;       // large member i's find jobs: find_first[i] .. find_first[i + 1] - 1
+  std::vector<Chain> chain;               // per large member
+  uint32_t n_rounds = 0;
+
+  void init(const Member *members, uint32_t n, uint64_t span) {
+    m.assign(members, members + n);
+    status.assign(n, MS_OK);
+    stored.clear(); small.clear(); large.clear(); find.clear(); chain.clear();
+    find_first.assign(1, 0);
+    n_rounds = 0;
+    for (uint32_t i = 0; i < n; i++) {
+      const Member &x = m[i];
+      if (x.method == 0) {
+        if (x.in_len != x.out_len) status[i] = MS_WRONG_SIZE;
+        else stored.push_back(i);
+      } else if (x.in_len <= span) {
+        SpanJob j{key_header(0), KEY_NONE, KEY_NONE, x.out_off, x.out_len, 1, 0, x.in_off, x.in_len, x.out_off, i, 0};
+        small.push_back(j);
+      } else {
+        large.push_back(i);
+        const uint32_t n_spans = (uint32_t)((x.in_len + span - 1) / span);
+        for (uint32_t k = 1; k < n_spans; k++) find.push_back(FindJob{x.in_off, x.in_len, k, 0});
+        find_first.push_back((uint32_t)find.size());
+      }
+    }
+  }
+  // cand: the find kernel's result, one key per entry of `find`
+  void start_chains(const uint64_t *cand, uint64_t span) {
+    chain.assign(large.size(), Chain());
+    std::vector<uint64_t> c;
+    for (size_t i = 0; i < large.size(); i++) {
+      const Member &x = m[large[i]];
+      const uint32_t n_spans = find_first[i + 1] - find_first[i] + 1;
+      c.assign(n_spans, KEY_NONE);
+      for (uint32_t k = 1; k < n_spans; k++) c[k] = cand[find_first[i] + k - 1];
+      chain[i].init(c.data(), n_spans, span, x.in_len, GIVE_UP_SPANS, x.in_off, large[i]);
+    }
+  }
+  // the spans of every unfinished chain to count in the next round: jobs[r] is span ref[r].second of chain ref[r].first
+  bool pending(std::vector<SpanJob> &jobs, std::vector<std::pair<uint32_t, uint32_t>> &ref) const {
+    jobs.clear();
+    ref.clear();
+    for (uint32_t i = 0; i < chain.size(); i++)
+      for (uint32_t s : chain[i].pending()) {
+        jobs.push_back(chain[i].job[s]);
+        ref.emplace_back(i, s);
+      }
+    return !jobs.empty();
+  }
+  void set_results(const std::vector<std::pair<uint32_t, uint32_t>> &ref, const SpanResult *res) {
+    n_rounds++;
+    std::vector<uint8_t> touched(chain.size(), 0);
+    for (size_t r = 0; r < ref.size(); r++) {
+      chain[ref[r].first].set_result(ref[r].second, res[r]);
+      touched[ref[r].first] = 1;
+    }
+    for (size_t i = 0; i < chain.size(); i++)
+      if (touched[i]) chain[i].advance();
+  }
+  // After the rounds: the decode jobs of every large member whose chain ended at its recorded size, member by member;
+  // first[i] .. first[i + 1] - 1 are the jobs of the i-th of them.  The others get their status here.
+  void layout(std::vector<SpanJob> &jobs, std::vector<uint32_t> &first) {
+    jobs.clear();
+    first.assign(1, 0);
+    for (size_t i = 0; i < chain.size(); i++) {
+      Chain &c = chain[i];
+      const uint32_t mi = large[i];
+      if (c.error || !c.done) { status[mi] = MS_BAD_DATA; continue; }
+      if (c.layout(m[mi].out_off) != m[mi].out_len) { status[mi] = MS_WRONG_SIZE; continue; }
+      jobs.insert(jobs.end(), c.job.begin(), c.job.end());
+      first.push_back((uint32_t)jobs.size());
+    }
+  }
+  uint32_t n_spans() const {
+    uint32_t s = 0;
+    for (const Chain &c : chain) s += (uint32_t)c.job.size();
+    return s;
+  }
+  uint32_t n_rejected() const {
+    uint32_t s = 0;
+    for (const Chain &c : chain) s += c.n_rejected;
+    return s;
+  }
+  uint32_t n_absorbed() const {
+    uint32_t s = 0;
+    for (const Chain &c : chain) s += c.n_absorbed;
+    return s;
+  }
+};
+// status of a one-span member from its decode
+IFL_HD int32_t member_status(int32_t span_status) {
+  return span_status == ST_OK ? MS_OK : span_status == ST_OVERFLOW ? MS_WRONG_SIZE : MS_BAD_DATA;
+}
 
 }  // namespace ifl
 }  // namespace lb2

@@ -16,11 +16,16 @@ last step of `lambdipy build` -- is wrapped: after the reference's copy, ./build
 (zipfile_gpu.zip_tree, the archive shutil.make_archive writes) and one line reports the zip against Lambda's 50 MB
 direct-upload limit and the tree against its 250 MB unzipped limit.
 
+With LAMBDIPY_BUNDLE_VERIFY=1 (default: unset, nothing changes) and LAMBDIPY_BUNDLE_ZIP set, the written bundle is
+read back on the GPU (zipfile_gpu.testzip: every member inflated and CRC-checked) before the size line; a bad member
+fails the build, and the line gains the member count.  No other value is accepted.
+
 With LAMBDIPY_DEFLATE_LEVEL=9 (default: unset, the default encoder) the GPU tarball mirror and the bundle zip use
 the thorough encoder (an optimal parse; smaller output, longer kernels).  No other value is accepted.
 """
 import os
 import sys
+import zipfile
 
 TARBALL_BACKENDS = ("python", "b200")
 UNTAR_BACKENDS = ("python", "b200")
@@ -47,8 +52,19 @@ def deflate_level():
     return 9
 
 
-def zip_after_copy(copy_include_paths, zip_path, compresslevel=None):
-    """copy_include_paths followed by the bundle zip of its build directory and the size line."""
+def bundle_verify():
+    """LAMBDIPY_BUNDLE_VERIFY, checked: False when unset, True for 1."""
+    v = os.environ.get("LAMBDIPY_BUNDLE_VERIFY")
+    if v is None:
+        return False
+    if v != "1":
+        raise ValueError("LAMBDIPY_BUNDLE_VERIFY=%r: expected 1 (check the bundle zip on the GPU) or unset" % v)
+    return True
+
+
+def zip_after_copy(copy_include_paths, zip_path, compresslevel=None, verify=False):
+    """copy_include_paths followed by the bundle zip of its build directory, with verify its read-back check, and the
+    size line."""
     def wrapped(include_paths, build_directory="./build"):
         copy_include_paths(include_paths, build_directory)
         from . import project_build, zipfile_gpu
@@ -56,10 +72,17 @@ def zip_after_copy(copy_include_paths, zip_path, compresslevel=None):
             zipfile_gpu.zip_tree(build_directory, zip_path)
         else:
             zipfile_gpu.zip_tree(build_directory, zip_path, compresslevel=compresslevel)
+        checked = ""
+        if verify:
+            bad = zipfile_gpu.testzip(zip_path)
+            if bad is not None:
+                raise RuntimeError("bundle zip %s: member %r does not read back (bad data, size or CRC-32)" % (zip_path, bad))
+            with zipfile.ZipFile(zip_path) as zf:
+                checked = "; %d members checked" % len(zf.infolist())
         zipped, unzipped = os.path.getsize(zip_path), project_build.tree_bytes(build_directory)
-        print("Bundle zip: %s, %.1f MB = %.0f %% of the 50 MB direct-upload limit; unzipped %.1f MB = %.0f %% of 250 MB"
+        print("Bundle zip: %s, %.1f MB = %.0f %% of the 50 MB direct-upload limit; unzipped %.1f MB = %.0f %% of 250 MB%s"
               % (zip_path, zipped / 1e6, 100.0 * zipped / LAMBDA_ZIPPED_LIMIT, unzipped / 1e6,
-                 100.0 * unzipped / project_build.LAMBDA_UNZIPPED_LIMIT))
+                 100.0 * unzipped / project_build.LAMBDA_UNZIPPED_LIMIT, checked))
     return wrapped
 
 
@@ -72,6 +95,7 @@ def apply():
         raise ValueError("LAMBDIPY_UNTAR_BACKEND=%r: expected one of %s" % (untar, ", ".join(UNTAR_BACKENDS)))
     zip_path = bundle_zip_path()
     level = deflate_level()
+    verify = bundle_verify()
     import lambdipy.cli as cli
     import lambdipy.project_build as ref
     from . import project_build as mine
@@ -85,7 +109,10 @@ def apply():
         from . import tarball
         ref.prepare_tarfile = tarball.prepare_tarfile
     if zip_path is not None:
-        cli.copy_include_paths = zip_after_copy(ref.copy_include_paths, zip_path, level)
+        if verify:
+            cli.copy_include_paths = zip_after_copy(ref.copy_include_paths, zip_path, level, verify=True)
+        else:
+            cli.copy_include_paths = zip_after_copy(ref.copy_include_paths, zip_path, level)
     # `lambdipy build` spends seconds resolving, downloading and copying packages before it reaches the
     # strip step (cli.py:52-67): create the CUDA context behind that, not in front of the strip
     if os.environ.get("LAMBDIPY_B200_EAGER_WARMUP", "1") != "0":

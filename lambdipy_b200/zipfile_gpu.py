@@ -1,4 +1,4 @@
-"""Lambda deployment zips with every member's DEFLATE body compressed on the GPU.
+"""Lambda deployment zips with every member's DEFLATE body compressed on the GPU, and zips read back on the GPU.
 
 A zip is the only package format AWS Lambda accepts, so the last step after `lambdipy build` is zipping `./build`,
 usually with `shutil.make_archive` or `zip -r`: zlib on one core over the whole bundle.
@@ -17,6 +17,13 @@ into the next piece is cut at a multiple of 64 KB of its bytes, so it is deflate
 
 The container is written here, with the standard library's `ZipInfo` for every local header.  The seam between the
 two is the encoder (`GpuZipEncoder`): anything with the same `buffers` / `submit` / `collect` can stand in for it.
+
+    extract_zip(zip_path, directory)  the tree `ZipFile(zip_path).extractall(directory)` writes
+    testzip(zip_path)                 the first bad member's name or None, as `ZipFile(zip_path).testzip()`
+
+read every STORED and DEFLATE member with the CUDA decoder behind `lb2_unzip_*` (csrc/inflate.cu): all members of a
+batch are inflated and CRC-checked in one pass, each bounded by its own body.  The seam there is the decoder
+(`GpuUnzipDecoder`).
 """
 import ctypes as C
 import os
@@ -301,3 +308,321 @@ def zip_tree(root_dir, zip_path, ctx=None, piece_bytes=PIECE_BYTES, compressleve
     finally:
         if own:
             ctx.close()
+
+
+# ---- reading: extract_zip / testzip ------------------------------------------------------------------------------
+# The central directory is parsed by the standard library (zip64, a prepended offset and data descriptors included);
+# each member's local header is read from the uploaded buffer to find its body, and every member the GPU can take is
+# decoded and CRC-checked by lb2_unzip_run.  The seam is the decoder (`GpuUnzipDecoder`): anything with the same
+# `buffer` / `run` / `stats` can stand in for it.
+
+BATCH_BYTES = 1 << 30   # archive bytes plus 3 bytes per output byte of one batch (the device memory it needs, at most)
+UNZIP_OK, UNZIP_BAD_DATA, UNZIP_WRONG_SIZE, UNZIP_BAD_CRC = 0, 1, 2, 3
+_GPU_METHODS = (zipfile.ZIP_STORED, zipfile.ZIP_DEFLATED)
+_STDLIB_FLAGS = 0x1 | 0x20 | 0x40   # encrypted, compressed patched data, strong encryption: the stdlib's own code
+
+
+class BadZipMember(zipfile.BadZipFile):
+    """A member whose DEFLATE data is invalid or truncated, or that decodes to another size than the archive records."""
+
+    def __init__(self, name, why):
+        super().__init__("%s for file %r" % (why, name))
+        self.member = name
+
+
+class DeviceTooSmall(Exception):
+    """The batch does not fit in device memory (lb2_unzip_run returned LB2_E_CAPACITY)."""
+
+
+class GpuUnzipDecoder:
+    """The lb2_unzip_* reader with a pinned input and output buffer.
+
+    buffer(n): a writable memoryview of n bytes, valid until the next buffer(); run(n, members) decodes
+    members [(body_off, body_len, size, crc32, method)] of buffer[:n] and returns [(status, data)] with status one of
+    UNZIP_* and data a memoryview of the member's bytes, valid until the next run(); DeviceTooSmall when the batch
+    does not fit on the device."""
+
+    def __init__(self, ctx):
+        self._ctx, self._u, self._in, self._out = ctx, None, None, None
+        self._in_cap = self._out_cap = 0
+        u = C.c_void_p()
+        ctx.check(ctx.lib.lb2_unzip_create(ctx.h, 0, C.byref(u)))
+        self._u = u
+        self._stats = {}
+
+    def _grow(self, attr, need):
+        cap = getattr(self, attr + "_cap")
+        if need <= cap:
+            return getattr(self, attr)
+        if getattr(self, attr) is not None:
+            self._ctx.pinned_free(getattr(self, attr))
+            setattr(self, attr, None)
+            setattr(self, attr + "_cap", 0)
+        cap = max(need, 2 * cap, 1 << 20)
+        setattr(self, attr, self._ctx.pinned_alloc(cap))
+        setattr(self, attr + "_cap", cap)
+        return getattr(self, attr)
+
+    def buffer(self, n):
+        p = self._grow("_in", n)
+        return memoryview((C.c_uint8 * n).from_address(p)).cast("B") if n else memoryview(bytearray())
+
+    def run(self, n, members):
+        k = len(members)
+        tab = (N.UnzipMember * max(k, 1))()
+        for i, (off, blen, size, crc, method) in enumerate(members):
+            tab[i].body_off, tab[i].body_len, tab[i].size, tab[i].crc32, tab[i].method = off, blen, size, crc, method
+        res, out_n, st = (N.UnzipResult * max(k, 1))(), C.c_uint64(), N.UnzipStats()
+        lib = self._ctx.lib
+        rc = lib.lb2_unzip_run(self._u, self._in if n else None, n, tab, k, C.byref(out_n), res, C.byref(st))
+        if rc == N.LB2_E_CAPACITY:
+            raise DeviceTooSmall((lib.lb2_last_error(self._ctx.h) or b"").decode())
+        self._ctx.check(rc)
+        p = self._grow("_out", out_n.value)
+        self._ctx.check(lib.lb2_unzip_read(self._u, p, out_n.value))
+        out = memoryview((C.c_uint8 * out_n.value).from_address(p)).cast("B") if out_n.value else memoryview(b"")
+        for key, v in st.as_dict().items():
+            self._stats[key] = self._stats.get(key, 0) + v
+        return [(res[i].status, out[res[i].out_off:res[i].out_off + members[i][2]]) for i in range(k)]
+
+    def stats(self):
+        d = dict(self._stats)
+        d["kernel_ms"] = sum(d.get(k, 0.0) for k in ("copy_ms", "small_ms", "find_ms", "count_ms", "decode_ms",
+                                                      "resolve_ms", "crc_ms"))
+        return d
+
+    def close(self):
+        if self._u is not None:
+            self._ctx.lib.lb2_unzip_destroy(self._u)
+            self._u = None
+        for attr in ("_in", "_out"):
+            if getattr(self, attr) is not None:
+                self._ctx.pinned_free(getattr(self, attr))
+                setattr(self, attr, None)
+                setattr(self, attr + "_cap", 0)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+def target_path(zf, member, path):
+    """Where ZipFile._extract_member (Python 3.12) puts `member` under `path`, its parent directories made: the name
+    with drive letters, absolute roots, "." and ".." dropped."""
+    arcname = member.filename.replace("/", os.path.sep)
+    if os.path.altsep:
+        arcname = arcname.replace(os.path.altsep, os.path.sep)
+    arcname = os.path.splitdrive(arcname)[1]
+    invalid_path_parts = ("", os.path.curdir, os.path.pardir)
+    arcname = os.path.sep.join(x for x in arcname.split(os.path.sep) if x not in invalid_path_parts)
+    if os.path.sep == "\\":
+        arcname = zf._sanitize_windows_name(arcname, os.path.sep)
+    if not arcname and not member.is_dir():
+        raise ValueError("Empty filename.")
+    targetpath = os.path.normpath(os.path.join(path, arcname))
+    upperdirs = os.path.dirname(targetpath)
+    if upperdirs and not os.path.exists(upperdirs):
+        os.makedirs(upperdirs)
+    return targetpath
+
+
+def _gpu_member(zi):
+    return zi.compress_type in _GPU_METHODS and not zi.flag_bits & _STDLIB_FLAGS and not zi.is_dir()
+
+
+def _body(zf, zi, buf, lo, archive_bytes):
+    """(offset of zi's body in buf, its length) after the checks ZipFile.open makes on the local header, or None when
+    a check fails (the stdlib's own code then raises what it raises)."""
+    off = zi.header_offset - lo
+    if off < 0 or off + zipfile.sizeFileHeader > len(buf):
+        return None
+    fh = struct.unpack(zipfile.structFileHeader, buf[off:off + zipfile.sizeFileHeader])
+    if fh[zipfile._FH_SIGNATURE] != zipfile.stringFileHeader:
+        return None
+    name_end = off + zipfile.sizeFileHeader + fh[zipfile._FH_FILENAME_LENGTH]
+    if name_end > len(buf):
+        return None
+    fname = bytes(buf[off + zipfile.sizeFileHeader:name_end])
+    try:
+        fname = fname.decode("utf-8" if fh[zipfile._FH_GENERAL_PURPOSE_FLAG_BITS] & 0x800 else
+                             (zf.metadata_encoding or "cp437"))
+    except UnicodeDecodeError:
+        return None
+    if fname != zi.orig_filename:
+        return None
+    body = name_end + fh[zipfile._FH_EXTRA_FIELD_LENGTH]
+    end_offset = getattr(zi, "_end_offset", None)
+    if end_offset is not None and lo + body + zi.compress_size > end_offset:
+        return None
+    if lo + body + zi.compress_size > archive_bytes:
+        return body, -1  # the file ends inside the body (ZipExtFile raises EOFError)
+    return body, zi.compress_size
+
+
+class _Reader:
+    """Decodes the GPU members of a run of entries, batch by batch, with the archive file's bytes read once."""
+
+    def __init__(self, zf, fp, decoder, batch_bytes):
+        self.zf, self.fp, self.decoder, self.batch_bytes = zf, fp, decoder, batch_bytes
+        fp.seek(0, os.SEEK_END)
+        self.archive_bytes = fp.tell()
+        self.n_gpu = self.n_stdlib = self.n_batches = 0
+        self.in_bytes = self.out_bytes = 0
+
+    def batches(self, entries):
+        """yield (entries of one batch, {id(ZipInfo): (status, data)} of its GPU members)"""
+        batch, cost = [], 0
+        for zi in entries:
+            c = zi.compress_size + 3 * zi.file_size + 1024
+            if batch and cost + c > self.batch_bytes:
+                yield batch, self.decode(batch)
+                batch, cost = [], 0
+            batch.append(zi)
+            cost += c
+        if batch:
+            yield batch, self.decode(batch)
+
+    def decode(self, batch):
+        todo = list({id(zi): zi for zi in batch if _gpu_member(zi)}.values())
+        got = {}
+        self._decode(todo, got)
+        self.n_batches += 1
+        return got
+
+    def _decode(self, todo, got):
+        if not todo:
+            return
+        lo = min(zi.header_offset for zi in todo)
+        hi = min(self.archive_bytes, max(zi.header_offset + zipfile.sizeFileHeader + 2 * 65535 + zi.compress_size
+                                         for zi in todo))
+        buf = self.decoder.buffer(max(hi - lo, 0))
+        self.fp.seek(lo)
+        _read_into(self.fp, buf)
+        members, infos = [], []
+        for zi in todo:
+            b = _body(self.zf, zi, buf, lo, self.archive_bytes)
+            if b is not None and b[1] < 0:
+                got[id(zi)] = (UNZIP_BAD_DATA, None)
+            elif b is not None:
+                members.append((b[0], b[1], zi.file_size, zi.CRC, zi.compress_type))
+                infos.append(zi)
+        try:
+            res = self.decoder.run(len(buf), members)
+        except DeviceTooSmall:
+            if len(infos) == 1:
+                return  # does not fit on the device alone: the stdlib's code reads it
+            half = len(infos) // 2
+            self._decode(infos[:half], got)
+            self._decode(infos[half:], got)
+            return
+        for zi, (status, data) in zip(infos, res):
+            got[id(zi)] = (status, bytes(data) if status == UNZIP_OK else None)
+            self.n_gpu += 1
+            self.in_bytes += zi.compress_size
+            self.out_bytes += zi.file_size
+
+    def stats(self, n_members):
+        st = {"members": n_members, "gpu_members": self.n_gpu, "batches": self.n_batches, "in_bytes": self.in_bytes,
+              "out_bytes": self.out_bytes}
+        st.update(self.decoder.stats())
+        return st
+
+
+def _raise_for(zi, status):
+    if status == UNZIP_BAD_CRC:
+        raise zipfile.BadZipFile("Bad CRC-32 for file %r" % zi.filename)
+    raise BadZipMember(zi.filename, "Invalid DEFLATE data" if status == UNZIP_BAD_DATA else "Wrong uncompressed size")
+
+
+def extract_with(zip_path, directory, decoder, batch_bytes=BATCH_BYTES):
+    """extract_zip with the member bodies decoded by `decoder` (GpuUnzipDecoder, or a stand-in with the same
+    interface)."""
+    path = os.fspath(directory)
+    with zipfile.ZipFile(zip_path) as zf, open(zip_path, "rb") as fp:
+        entries = [zf.getinfo(name) for name in zf.namelist()]  # as extractall: a repeated name is its last entry
+        r = _Reader(zf, fp, decoder, batch_bytes)
+        n_files = n_stdlib = 0
+        for batch, got in r.batches(entries):
+            for zi in batch:  # the whole batch is checked before any of its files is written
+                status = got.get(id(zi), (UNZIP_OK, None))[0]
+                if status != UNZIP_OK:
+                    _raise_for(zi, status)
+            for zi in batch:
+                if id(zi) in got:
+                    with open(target_path(zf, zi, path), "wb") as f:
+                        f.write(got[id(zi)][1])
+                    n_files += 1
+                else:
+                    n_stdlib += not zi.is_dir()
+                    zf.extract(zi, path)
+    st = r.stats(len(entries))
+    st.update(files=n_files, stdlib_members=n_stdlib)
+    return st
+
+
+def testzip_with(zip_path, decoder, batch_bytes=BATCH_BYTES):
+    """testzip with the member bodies decoded by `decoder`; returns (name or None, stats)."""
+    with zipfile.ZipFile(zip_path) as zf, open(zip_path, "rb") as fp:
+        listed = list(zf.filelist)
+        byname = {id(zi): zf.getinfo(zi.filename) for zi in listed}  # ZipFile.testzip opens each entry by its name
+        r = _Reader(zf, fp, decoder, batch_bytes)
+        pos = 0
+        n_stdlib = 0
+        for batch, got in r.batches([byname[id(zi)] for zi in listed]):
+            for zi in batch:
+                name = listed[pos].filename
+                pos += 1
+                if id(zi) in got:
+                    if got[id(zi)][0] != UNZIP_OK:
+                        return name, r.stats(len(listed))
+                    continue
+                n_stdlib += not zi.is_dir()
+                try:
+                    with zf.open(zi, "r") as f:
+                        while f.read(1 << 20):
+                            pass
+                except zipfile.BadZipFile:
+                    return name, r.stats(len(listed))
+    st = r.stats(len(listed))
+    st["stdlib_members"] = n_stdlib
+    return None, st
+
+
+def _with_decoder(ctx, fn):
+    from .tarball import _default_context
+    own = False
+    if ctx is None:
+        ctx, own = _default_context()
+    try:
+        with GpuUnzipDecoder(ctx) as dec:
+            return fn(dec)
+    finally:
+        if own:
+            ctx.close()
+
+
+def extract_zip(zip_path, directory, ctx=None, batch_bytes=BATCH_BYTES):
+    """Extract `zip_path` under `directory` as `ZipFile(zip_path).extractall(directory)` does -- the same paths (".."
+    components, drive letters and absolute names sanitised as its _extract_member does), directories and contents,
+    in archive order -- with every STORED and DEFLATE member decoded and CRC-checked on the GPU.  Members are decoded
+    in batches bounded by device memory; a batch is decoded and checked before any of its files is written.
+
+    A CRC mismatch raises zipfile.BadZipFile("Bad CRC-32 for file %r"), as the stdlib does; invalid DEFLATE data or a
+    wrong size raises BadZipMember (a BadZipFile) naming the member.  Encrypted members, other methods (bzip2, lzma,
+    deflate64), members whose local header the stdlib would refuse and members that do not fit on the device alone
+    are extracted by the stdlib's own code.  Returns a stats dict: members, gpu_members, stdlib_members, files,
+    batches, in_bytes, out_bytes, kernel_ms and the lb2_unzip_stats fields summed over the batches.  ctx=None: the
+    context the strip path has already warmed up, if any, else a new one.  There is no CPU path: without a GPU this
+    raises."""
+    return _with_decoder(ctx, lambda dec: extract_with(zip_path, directory, dec, batch_bytes))
+
+
+def testzip(zip_path, ctx=None, batch_bytes=BATCH_BYTES):
+    """The name of the first bad member of `zip_path`, or None, as `ZipFile(zip_path).testzip()` returns it, with
+    every STORED and DEFLATE member decoded and CRC-checked on the GPU.  One difference: where the stdlib raises
+    instead of naming the member -- zlib.error for invalid DEFLATE data, EOFError for a body cut short by its recorded
+    sizes -- this returns the member's name.  (A member that decodes to fewer bytes than its recorded size is also
+    named; the stdlib passes it when the CRC-32 of the shorter output matches.)"""
+    return _with_decoder(ctx, lambda dec: testzip_with(zip_path, dec, batch_bytes)[0])
