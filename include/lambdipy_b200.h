@@ -17,7 +17,9 @@
  *   lb2_strip_host()          == `strip` over a batch of files already read into host memory
  *                                (what xargs hands to one strip process), results to host memory.
  *   lb2_strip_device_async()  == the same batch with input and output arenas resident in HBM
- *                                (benchmark / pipeline building block).
+ *                                (benchmark / pipeline building block; with lb2_unzip_device_output in front
+ *                                and lb2_zip_submit_device behind it, the same line applied to the "*.so"
+ *                                members of a zip without unpacking it).
  *
  * Result contract: for every file with status LB2_ST_OK the output bytes are identical to
  * `strip --strip-unneeded -o OUT IN` of GNU Binutils 2.42 (== flagless `strip` for ET_DYN/ET_EXEC).
@@ -240,7 +242,7 @@ typedef struct lb2_gzip_stats {
   uint32_t n_chunks, n_stored_chunks, n_fixed_chunks;  /* 64 KB chunks; those written stored / fixed Huffman */
   float deflate_ms;                  /* deflate + compaction kernels, CUDA events, summed over pieces */
   float crc_ms;                      /* CRC-32 kernel                                                 */
-  float h2d_ms;                      /* piece uploads (CUDA events)                                   */
+  float h2d_ms;                      /* piece uploads, or the gathers of device pieces (CUDA events)  */
   float d2h_ms;                      /* result downloads (host clock around the copy)                 */
   uint32_t n_opt_chunks;             /* chunks written from the optimal parse (0 in the default mode) */
   float best_ms;                     /* best mode: the optimal-parse kernel (also in deflate_ms)      */
@@ -299,6 +301,20 @@ int lb2_zip_submit(lb2_zip *z, const void *h_in, uint64_t n, const uint64_t *seg
 /* LB2_E_CAPACITY when out_cap is too small: *out_n says how much is needed, the piece stays in flight */
 int lb2_zip_collect(lb2_zip *z, void *h_out, uint64_t out_cap, uint64_t *out_n, lb2_zip_segment *segs,
                     lb2_gzip_stats *stats);
+/* A piece whose segments are already in device memory -- the output of lb2_unzip_run or of a strip call, which is how
+ * zipfile_gpu.strip_zip strips the shared objects inside a zip (what `extractall`, the reference's
+ * `find -name "*.so" | xargs strip` and `make_archive` do in three passes over the file system) without the decoded
+ * bytes leaving the device.  Segment i is src[i].len bytes at src[i].d_ptr, of any alignment.  A gather kernel on the
+ * writer's stream lays the segments out at 16-byte-aligned offsets of the piece, in order, and zeroes the gaps; from
+ * there the piece is what lb2_zip_submit makes of the same segments -- the same chunks, history, flags, states and
+ * LB2_E_STATE cases, collected by lb2_zip_collect, with the same bytes out (stats.h2d_ms then times the gather).
+ * The caller guarantees that the sources are complete when this is called (lb2_unzip_run and lb2_batch_results both
+ * end in a host wait) and leaves them unchanged until the piece is collected. */
+typedef struct lb2_zip_source {
+  const void *d_ptr;           /* device memory                                                             */
+  uint64_t len;                /* bytes; 0 for an empty file (d_ptr may then be NULL)                       */
+} lb2_zip_source;
+int lb2_zip_submit_device(lb2_zip *z, const lb2_zip_source *src, uint32_t n_segs, uint32_t flags);
 void lb2_zip_destroy(lb2_zip *z);
 
 /* ---- gzip reader: raw DEFLATE (RFC 1951) decoded on the GPU ----------------------------------- */
@@ -384,6 +400,11 @@ int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_me
                   uint64_t *out_n, lb2_unzip_result *results, lb2_unzip_stats *stats);
 /* copy the output of the last successful run to h_out (cap >= *out_n) */
 int lb2_unzip_read(lb2_unzip *u, void *h_out, uint64_t cap);
+/* The device buffer lb2_unzip_read would copy from, *n bytes at *d_out (NULL when *n is 0): member i's bytes are at
+ * results[i].out_off, a multiple of 16, which is what lb2_strip_device_async wants of an input arena and what
+ * lb2_zip_submit_device takes as a source.  Valid until the next lb2_unzip_run or lb2_unzip_destroy.  LB2_E_STATE
+ * without a successful run. */
+int lb2_unzip_device_output(lb2_unzip *u, const void **d_out, uint64_t *n);
 void lb2_unzip_destroy(lb2_unzip *u);
 
 #ifdef __cplusplus

@@ -28,6 +28,7 @@ EXPORTS = [
     "lb2_inflate_create", "lb2_inflate_run", "lb2_inflate_read", "lb2_inflate_destroy",
     "lb2_zip_create", "lb2_zip_submit", "lb2_zip_collect", "lb2_zip_destroy",
     "lb2_unzip_create", "lb2_unzip_run", "lb2_unzip_read", "lb2_unzip_destroy",
+    "lb2_zip_submit_device", "lb2_unzip_device_output",
 ]
 ZIP_CONTINUES, ZIP_MORE = 1, 2
 DEFLATE_BEST = 1  # LB2_DEFLATE_BEST
@@ -95,6 +96,10 @@ def zip_bound(n, n_segs):
 
 class ZipSegment(C.Structure):
     _fields_ = [("out_off", C.c_uint64), ("out_len", C.c_uint64), ("crc32", C.c_uint32), ("ended", C.c_uint32)]
+
+
+class ZipSource(C.Structure):
+    _fields_ = [("d_ptr", C.c_void_p), ("len", C.c_uint64)]
 
 
 class InflateStats(C.Structure):
@@ -227,6 +232,8 @@ def load():
     lib.lb2_zip_create.restype = C.c_int
     lib.lb2_zip_submit.argtypes = [vp, vp, C.c_uint64, u64p, u64p, C.c_uint32, C.c_uint32]
     lib.lb2_zip_submit.restype = C.c_int
+    lib.lb2_zip_submit_device.argtypes = [vp, C.POINTER(ZipSource), C.c_uint32, C.c_uint32]
+    lib.lb2_zip_submit_device.restype = C.c_int
     lib.lb2_zip_collect.argtypes = [vp, vp, C.c_uint64, u64p, C.POINTER(ZipSegment), C.POINTER(GzipStats)]
     lib.lb2_zip_collect.restype = C.c_int
     lib.lb2_zip_destroy.argtypes = [vp]
@@ -238,6 +245,8 @@ def load():
     lib.lb2_unzip_run.restype = C.c_int
     lib.lb2_unzip_read.argtypes = [vp, vp, C.c_uint64]
     lib.lb2_unzip_read.restype = C.c_int
+    lib.lb2_unzip_device_output.argtypes = [vp, C.POINTER(vp), u64p]
+    lib.lb2_unzip_device_output.restype = C.c_int
     lib.lb2_unzip_destroy.argtypes = [vp]
     lib.lb2_unzip_destroy.restype = None
     _lib = lib

@@ -485,7 +485,8 @@ struct GzSlot {
   uint8_t *d_tab = nullptr, *h_tab = nullptr;    // GzChunk[n_chunks] then GzSeg[n_segs]
   GzSegResult *d_seg = nullptr, *h_seg = nullptr;  // per-segment results (lb2_zip_segment layout)
   GzResult *d_res = nullptr, *h_res = nullptr;
-  uint64_t cap_bytes = 0, cap_tab = 0;
+  GzGatherTile *d_gat = nullptr, *h_gat = nullptr;  // lb2_zip_submit_device: the tiles that lay the piece out in d_in
+  uint64_t cap_bytes = 0, cap_tab = 0, cap_gat = 0;
   uint32_t cap_chunks = 0, cap_segs = 0;
   cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // upload | deflate | best | crc | compact |
   cudaEvent_t done = nullptr;
@@ -511,8 +512,9 @@ struct lb2_zip : GzWriter {};
 
 static void gz_slot_free(GzSlot &s) {
   cudaFree(s.d_in); cudaFree(s.d_chunk_out); cudaFree(s.d_out); cudaFree(s.d_tok); cudaFree(s.d_meta); cudaFree(s.d_off);
-  cudaFree(s.d_tab); cudaFree(s.d_seg); cudaFree(s.d_res);
+  cudaFree(s.d_tab); cudaFree(s.d_seg); cudaFree(s.d_res); cudaFree(s.d_gat);
   if (s.h_tab) cudaFreeHost(s.h_tab);
+  if (s.h_gat) cudaFreeHost(s.h_gat);
   if (s.h_seg) cudaFreeHost(s.h_seg);
   if (s.h_res) cudaFreeHost(s.h_res);
   for (auto &e : s.ev) if (e) cudaEventDestroy(e);
@@ -592,10 +594,11 @@ static void gz_destroy(GzWriter *g) {
   if (g->stream) cudaStreamDestroy(g->stream);
 }
 
-// Enqueue one piece of n bytes at h_in holding n_segs segments [seg_off[i], seg_off[i] + seg_len[i]) (validated by
-// the caller).  cont: segment 0 continues the open stream / file; ends: segment i's file ends in this piece.
-static int gz_submit(GzWriter *g, const void *h_in, uint64_t n, const uint64_t *seg_off, const uint64_t *seg_len,
-                     uint32_t n_segs, bool cont, bool last_ends) {
+// Enqueue one piece of n bytes holding n_segs segments [seg_off[i], seg_off[i] + seg_len[i]) (validated by the
+// caller).  The piece is uploaded from h_in, or, when d_src is given, gathered on the device: segment i is seg_len[i]
+// bytes at d_src[i].d_ptr.  cont: segment 0 continues the open stream / file; ends: segment i's file ends in this piece.
+static int gz_submit(GzWriter *g, const void *h_in, const lb2_zip_source *d_src, uint64_t n, const uint64_t *seg_off,
+                     const uint64_t *seg_len, uint32_t n_segs, bool cont, bool last_ends) {
   lb2_ctx *ctx = g->ctx;
   CK(cudaSetDevice(ctx->device));
   GzSlot &s = g->slot[(g->head + g->count) & 1];
@@ -604,6 +607,28 @@ static int gz_submit(GzWriter *g, const void *h_in, uint64_t n, const uint64_t *
   if (n_chunks > UINT32_MAX / 2) { ctx->err = "piece too large"; return LB2_E_ARG; }
   int rc = gz_slot_reserve(ctx, s, n, (uint32_t)n_chunks, n_segs);
   if (rc) return rc;
+  uint64_t n_tiles = 0;
+  if (d_src) {
+    for (uint32_t i = 0; i < n_segs; i++) n_tiles += (seg_len[i] + GZ_GATHER_TILE - 1) / GZ_GATHER_TILE;
+    if (n_tiles > s.cap_gat) {
+      const uint64_t t = std::max(n_tiles, 2 * s.cap_gat);
+      cudaFree(s.d_gat);
+      if (s.h_gat) cudaFreeHost(s.h_gat);
+      s.d_gat = s.h_gat = nullptr;
+      s.cap_gat = 0;
+      CK(cudaMalloc(&s.d_gat, t * sizeof(GzGatherTile)));
+      CK(cudaHostAlloc(&s.h_gat, t * sizeof(GzGatherTile), cudaHostAllocDefault));
+      s.cap_gat = t;
+    }
+    GzGatherTile *tile = s.h_gat;
+    for (uint32_t i = 0; i < n_segs; i++)
+      for (uint64_t p = 0; p < seg_len[i]; p += GZ_GATHER_TILE) {
+        const uint32_t len = (uint32_t)std::min<uint64_t>(GZ_GATHER_TILE, seg_len[i] - p);
+        const uint64_t end = seg_off[i] + p + len;
+        *tile++ = GzGatherTile{static_cast<const uint8_t *>(d_src[i].d_ptr) + p, seg_off[i] + p, len,
+                               p + len == seg_len[i] ? (uint32_t)(-end & 15) : 0u};
+      }
+  }
   GzChunk *chunks = reinterpret_cast<GzChunk *>(s.h_tab);
   GzSeg *segs = reinterpret_cast<GzSeg *>(s.h_tab + n_chunks * sizeof(GzChunk));
   uint32_t c = 0, n_data = 0;
@@ -633,7 +658,12 @@ static int gz_submit(GzWriter *g, const void *h_in, uint64_t n, const uint64_t *
   CK(cudaEventRecord(s.ev[0], st));
   if (cont && g->hist_len)
     CK(cudaMemcpyAsync(s.d_in + GZ_HIST - g->hist_len, g->d_hist, g->hist_len, cudaMemcpyDeviceToDevice, st));
-  if (n) CK(cudaMemcpyAsync(s.d_in + GZ_HIST, h_in, n, cudaMemcpyHostToDevice, st));
+  if (d_src) {
+    if (n_tiles) CK(cudaMemcpyAsync(s.d_gat, s.h_gat, n_tiles * sizeof(GzGatherTile), cudaMemcpyHostToDevice, st));
+    launch_zip_gather(s.d_gat, (uint32_t)n_tiles, s.d_in + GZ_HIST, st);
+  } else if (n) {
+    CK(cudaMemcpyAsync(s.d_in + GZ_HIST, h_in, n, cudaMemcpyHostToDevice, st));
+  }
   CK(cudaMemcpyAsync(s.d_tab, s.h_tab, n_chunks * sizeof(GzChunk) + n_segs * sizeof(GzSeg), cudaMemcpyHostToDevice, st));
   CK(cudaEventRecord(s.ev[1], st));
   launch_deflate(a, st);
@@ -732,7 +762,7 @@ int lb2_gzip_submit(lb2_gzip *g, const void *h_in, uint64_t n) {
   }
   // the piece is one segment of the stream, which continues from the previous piece and stays open
   const uint64_t off = 0;
-  return gz_submit(g, h_in, n, &off, &n, 1, true, false);
+  return gz_submit(g, h_in, nullptr, n, &off, &n, 1, true, false);
 }
 
 int lb2_gzip_collect(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n) {
@@ -782,18 +812,27 @@ void lb2_zip_destroy(lb2_zip *z) {
   delete z;
 }
 
+// the checks lb2_zip_submit and lb2_zip_submit_device share, made before the segments are looked at
+static int zip_submit_checks(lb2_zip *z, uint32_t n_segs, uint32_t flags) {
+  lb2_ctx *ctx = z->ctx;
+  if (flags & ~(LB2_ZIP_CONTINUES | LB2_ZIP_MORE)) { ctx->err = "lb2_zip_submit: unknown flags"; return LB2_E_ARG; }
+  if (!n_segs) { ctx->err = "a piece holds at least one segment"; return LB2_E_ARG; }
+  if (z->count >= 2) { ctx->err = "two pieces already in flight: collect one with lb2_zip_collect first"; return LB2_E_STATE; }
+  const bool cont = flags & LB2_ZIP_CONTINUES;
+  if (cont && !z->open) { ctx->err = "LB2_ZIP_CONTINUES, but the previous piece left no file open"; return LB2_E_STATE; }
+  if (!cont && z->open) { ctx->err = "the previous piece's last file is still open: continue it with LB2_ZIP_CONTINUES"; return LB2_E_STATE; }
+  return LB2_OK;
+}
+
 int lb2_zip_submit(lb2_zip *z, const void *h_in, uint64_t n, const uint64_t *seg_off, const uint64_t *seg_len, uint32_t n_segs,
                    uint32_t flags) {
   if (!z) return LB2_E_ARG;
   lb2_ctx *ctx = z->ctx;
   if ((!h_in && n) || !seg_off || !seg_len) { ctx->err = "NULL argument"; return LB2_E_ARG; }
-  if (flags & ~(LB2_ZIP_CONTINUES | LB2_ZIP_MORE)) { ctx->err = "lb2_zip_submit: unknown flags"; return LB2_E_ARG; }
-  if (!n_segs) { ctx->err = "a piece holds at least one segment"; return LB2_E_ARG; }
   if (n > (uint64_t)UINT32_MAX * GZ_CHUNK / 2) { ctx->err = "piece too large"; return LB2_E_ARG; }
-  if (z->count >= 2) { ctx->err = "two pieces already in flight: collect one with lb2_zip_collect first"; return LB2_E_STATE; }
+  const int rc = zip_submit_checks(z, n_segs, flags);
+  if (rc) return rc;
   const bool cont = flags & LB2_ZIP_CONTINUES;
-  if (cont && !z->open) { ctx->err = "LB2_ZIP_CONTINUES, but the previous piece left no file open"; return LB2_E_STATE; }
-  if (!cont && z->open) { ctx->err = "the previous piece's last file is still open: continue it with LB2_ZIP_CONTINUES"; return LB2_E_STATE; }
   if (cont && seg_off[0]) { ctx->err = "a continued file starts the piece: seg_off[0] must be 0"; return LB2_E_ARG; }
   uint64_t end = 0;
   for (uint32_t i = 0; i < n_segs; i++) {
@@ -803,7 +842,25 @@ int lb2_zip_submit(lb2_zip *z, const void *h_in, uint64_t n, const uint64_t *seg
     }
     end = seg_off[i] + seg_len[i];
   }
-  return gz_submit(z, h_in, n, seg_off, seg_len, n_segs, cont, !(flags & LB2_ZIP_MORE));
+  return gz_submit(z, h_in, nullptr, n, seg_off, seg_len, n_segs, cont, !(flags & LB2_ZIP_MORE));
+}
+
+int lb2_zip_submit_device(lb2_zip *z, const lb2_zip_source *src, uint32_t n_segs, uint32_t flags) {
+  if (!z) return LB2_E_ARG;
+  lb2_ctx *ctx = z->ctx;
+  if (!src) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  const int rc = zip_submit_checks(z, n_segs, flags);
+  if (rc) return rc;
+  std::vector<uint64_t> off(n_segs), len(n_segs);
+  uint64_t n = 0;  // the piece: every segment at the next multiple of 16
+  for (uint32_t i = 0; i < n_segs; i++) {
+    if (!src[i].d_ptr && src[i].len) { ctx->err = "segment " + std::to_string(i) + ": NULL source"; return LB2_E_ARG; }
+    off[i] = (n + 15) & ~15ull;
+    len[i] = src[i].len;
+    if (len[i] > (uint64_t)UINT32_MAX * GZ_CHUNK / 2 - off[i]) { ctx->err = "piece too large"; return LB2_E_ARG; }
+    n = off[i] + len[i];
+  }
+  return gz_submit(z, nullptr, src, n, off.data(), len.data(), n_segs, flags & LB2_ZIP_CONTINUES, !(flags & LB2_ZIP_MORE));
 }
 
 int lb2_zip_collect(lb2_zip *z, void *h_out, uint64_t out_cap, uint64_t *out_n, lb2_zip_segment *segs, lb2_gzip_stats *stats) {
@@ -1274,6 +1331,16 @@ int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_me
   u->out_n = total;
   u->have = true;
   *out_n = total;
+  return LB2_OK;
+}
+
+int lb2_unzip_device_output(lb2_unzip *u, const void **d_out, uint64_t *n) {
+  if (!u) return LB2_E_ARG;
+  lb2_ctx *ctx = u->ctx;
+  if (!d_out || !n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if (!u->have) { ctx->err = "lb2_unzip_device_output: no decoded batch (lb2_unzip_run failed or was not called)"; return LB2_E_STATE; }
+  *d_out = u->d_out;
+  *n = u->out_n;
   return LB2_OK;
 }
 

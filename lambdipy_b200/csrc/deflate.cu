@@ -925,6 +925,17 @@ __global__ void __launch_bounds__(256) lb2_gzip_gather_kernel(GzPieceArgs a) {
   warp_copy_tile(a.chunk_out + a.chunks[c].start + (uint64_t)c * GZ_OUT_PAD, a.out + a.chunk_off[c], a.chunk_size[c], lane);
 }
 
+// The same on the input side, for a piece whose segments are already in device memory: one warp per tile of a segment,
+// source and destination of any relative alignment, and the padding behind a segment zeroed.
+__global__ void __launch_bounds__(256) lb2_zip_gather_kernel(const GzGatherTile *tiles, uint32_t n_tiles, uint8_t *in) {
+  const uint32_t t = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (t >= n_tiles) return;
+  const int lane = threadIdx.x & 31;
+  const GzGatherTile g = tiles[t];
+  warp_copy_tile(g.src, in + g.dst, g.len, lane);
+  if (lane < (int)g.pad) in[g.dst + g.len + lane] = 0;
+}
+
 }  // namespace
 
 void launch_deflate(const GzPieceArgs &a, cudaStream_t s) {
@@ -955,6 +966,9 @@ void launch_segment_crc32(const GzPieceArgs &a, cudaStream_t s) {
 void launch_gzip_compact(const GzPieceArgs &a, cudaStream_t s) {
   lb2_gzip_scan_kernel<<<1, SCAN_THREADS, 0, s>>>(a);
   lb2_gzip_gather_kernel<<<(a.n_chunks + 7) / 8, 256, 0, s>>>(a);
+}
+void launch_zip_gather(const GzGatherTile *tiles, uint32_t n_tiles, uint8_t *in, cudaStream_t s) {
+  if (n_tiles) lb2_zip_gather_kernel<<<(n_tiles + 7) / 8, 256, 0, s>>>(tiles, n_tiles, in);
 }
 
 }  // namespace lb2

@@ -24,10 +24,22 @@ two is the encoder (`GpuZipEncoder`): anything with the same `buffers` / `submit
 read every STORED and DEFLATE member with the CUDA decoder behind `lb2_unzip_*` (csrc/inflate.cu): all members of a
 batch are inflated and CRC-checked in one pass, each bounded by its own body.  The seam there is the decoder
 (`GpuUnzipDecoder`).
+
+    strip_zip(src_zip, dst_zip)       the zip `extractall`, the reference's `find -name "*.so" | xargs strip` and
+                                      `make_archive` would make of src_zip, members and order kept
+
+chains the three engines on the device: the `*.so` members are inflated by the decoder, stripped where they lie by
+the strip kernels (`GpuStripper`) and deflated by the encoder straight from the stripped arena
+(`lb2_zip_submit_device`); every other member's body is copied from src_zip as it is.
+`python -m lambdipy_b200.zipfile_gpu strip SRC DST [--level 9]` is the same call from a shell.
 """
+import copy
 import ctypes as C
 import os
 import struct
+import subprocess
+import sys
+import tempfile
 import zipfile
 
 from . import _native as N
@@ -44,9 +56,12 @@ class GpuZipEncoder:
     buffers[k]: writable memoryview of piece_bytes; submit(k, n, seg_off, seg_len, flags) hands buffers[k][:n] to the
     GPU (flags: N.ZIP_CONTINUES / N.ZIP_MORE); collect() waits for the oldest piece and returns (its DEFLATE bytes,
     [(out_off, out_len, crc32, ended) per segment]); the bytes stay valid until the next collect().
-    compresslevel: None (the default encoder) or 9 (the optimal parse, LB2_DEFLATE_BEST)."""
+    compresslevel: None (the default encoder) or 9 (the optimal parse, LB2_DEFLATE_BEST).
 
-    def __init__(self, ctx, piece_bytes=PIECE_BYTES, max_segs=MAX_SEGS, compresslevel=None):
+    submit_device(refs, flags) hands over a piece whose segments are (device address, length) pairs instead, laid out
+    by the library (lb2_zip_submit_device); a writer fed only that way needs no piece buffers (host_buffers=False)."""
+
+    def __init__(self, ctx, piece_bytes=PIECE_BYTES, max_segs=MAX_SEGS, compresslevel=None, host_buffers=True):
         flags = N.deflate_flags(compresslevel)  # checked before anything is allocated
         self._ctx, self._z, self._ptrs, self._out = ctx, None, [], None
         self.piece_bytes, self.max_segs = int(piece_bytes), int(max_segs)
@@ -55,7 +70,7 @@ class GpuZipEncoder:
             ctx.check(ctx.lib.lb2_zip_create(ctx.h, flags, C.byref(z)))
             self._z = z
             self.buffers = []
-            for _ in range(2):
+            for _ in range(2 if host_buffers else 0):
                 p = ctx.pinned_alloc(self.piece_bytes)
                 self._ptrs.append(p)
                 self.buffers.append(memoryview((C.c_uint8 * self.piece_bytes).from_address(p)).cast("B"))
@@ -71,6 +86,14 @@ class GpuZipEncoder:
         ns = len(seg_off)
         offs, lens = (C.c_uint64 * ns)(*seg_off), (C.c_uint64 * ns)(*seg_len)
         self._ctx.check(self._ctx.lib.lb2_zip_submit(self._z, self._ptrs[k], n, offs, lens, ns, flags))
+        self._pending.append(ns)
+
+    def submit_device(self, refs, flags):
+        ns = len(refs)
+        src = (N.ZipSource * ns)()
+        for i, (addr, n) in enumerate(refs):
+            src[i].d_ptr, src[i].len = addr, n
+        self._ctx.check(self._ctx.lib.lb2_zip_submit_device(self._z, src, ns, flags))
         self._pending.append(ns)
 
     def collect(self):
@@ -121,9 +144,10 @@ def tree_entries(root_dir):
     return entries
 
 
-def central_directory(infos, start):
+def central_directory(infos, start, comment=b""):
     """The central directory of `infos` (written from offset `start`) and the end records, as ZipFile.close() writes
-    them: zip64 extras for sizes or offsets beyond ZIP64_LIMIT, zip64 end records beyond 65 535 entries or 4 GiB."""
+    them: zip64 extras for sizes or offsets beyond ZIP64_LIMIT, zip64 end records beyond 65 535 entries or 4 GiB, then
+    the archive comment."""
     out = []
     for zi in infos:
         dt = zi.date_time
@@ -158,26 +182,32 @@ def central_directory(infos, start):
                           0, 0, count, count, size, offset)
         cd += struct.pack(zipfile.structEndArchive64Locator, zipfile.stringEndArchive64Locator, 0, start + size, 1)
         count, size, offset = min(count, 0xFFFF), min(size, 0xFFFFFFFF), min(offset, 0xFFFFFFFF)
-    return cd + struct.pack(zipfile.structEndArchive, zipfile.stringEndArchive, 0, 0, count, count, size, offset, 0)
+    return cd + struct.pack(zipfile.structEndArchive, zipfile.stringEndArchive, 0, 0, count, count, size, offset,
+                            len(comment)) + comment
 
 
 class _ContainerWriter:
     """Writes the entries in order as their bodies arrive: a directory as soon as every entry before it is written;
     a file's local header when its first body bytes arrive, rewritten with the CRC and sizes once it ends (seeking
-    back, as ZipFile does on a seekable file)."""
+    back, as ZipFile does on a seekable file).  With `copy` (strip_zip), an entry whose body never arrives is not a
+    directory of the tree but a member kept as it is: copy(ZipInfo) writes its header and body at the current
+    position."""
 
-    def __init__(self, fp, entries):
-        self.fp, self.entries, self.next = fp, entries, 0
+    def __init__(self, fp, entries, copy=None):
+        self.fp, self.entries, self.next, self.copy = fp, entries, 0, copy
         self.cur = None  # (ZipInfo, zip64) of the file being written
         self.in_bytes = self.out_bytes = self.n_files = 0
 
     def _upto(self, idx):
         while self.next < idx:
             zi = self.entries[self.next][1]
-            assert zi.is_dir(), "file entry %s written out of order" % zi.filename
-            zi.compress_size = zi.CRC = 0
             zi.header_offset = self.fp.tell()
-            self.fp.write(zi.FileHeader(False))
+            if self.copy is not None:
+                self.copy(zi)
+            else:
+                assert zi.is_dir(), "file entry %s written out of order" % zi.filename
+                zi.compress_size = zi.CRC = 0
+                self.fp.write(zi.FileHeader(False))
             self.next += 1
 
     def part(self, idx, body, crc, ended, file_bytes):
@@ -211,10 +241,10 @@ class _ContainerWriter:
             self.cur = None
             self.next = idx + 1
 
-    def finish(self):
+    def finish(self, comment=b""):
         self._upto(len(self.entries))
         start = self.fp.tell()
-        self.fp.write(central_directory([zi for _, zi in self.entries], start))
+        self.fp.write(central_directory([zi for _, zi in self.entries], start, comment))
 
 
 def _read_into(f, view):
@@ -367,7 +397,7 @@ class GpuUnzipDecoder:
         p = self._grow("_in", n)
         return memoryview((C.c_uint8 * n).from_address(p)).cast("B") if n else memoryview(bytearray())
 
-    def run(self, n, members):
+    def run(self, n, members, device=False):
         k = len(members)
         tab = (N.UnzipMember * max(k, 1))()
         for i, (off, blen, size, crc, method) in enumerate(members):
@@ -378,12 +408,21 @@ class GpuUnzipDecoder:
         if rc == N.LB2_E_CAPACITY:
             raise DeviceTooSmall((lib.lb2_last_error(self._ctx.h) or b"").decode())
         self._ctx.check(rc)
+        for key, v in st.as_dict().items():
+            self._stats[key] = self._stats.get(key, 0) + v
+        if device:
+            d_out, d_n = C.c_void_p(), C.c_uint64()
+            self._ctx.check(lib.lb2_unzip_device_output(self._u, C.byref(d_out), C.byref(d_n)))
+            return [(res[i].status, ((d_out.value or 0) + res[i].out_off, members[i][2])) for i in range(k)]
         p = self._grow("_out", out_n.value)
         self._ctx.check(lib.lb2_unzip_read(self._u, p, out_n.value))
         out = memoryview((C.c_uint8 * out_n.value).from_address(p)).cast("B") if out_n.value else memoryview(b"")
-        for key, v in st.as_dict().items():
-            self._stats[key] = self._stats.get(key, 0) + v
         return [(res[i].status, out[res[i].out_off:res[i].out_off + members[i][2]]) for i in range(k)]
+
+    def run_device(self, n, members):
+        """run() with the decoded members left on the device: [(status, (device address, size))], the addresses
+        multiples of 16 inside one buffer and valid until the next run."""
+        return self.run(n, members, device=True)
 
     def stats(self):
         d = dict(self._stats)
@@ -626,3 +665,389 @@ def testzip(zip_path, ctx=None, batch_bytes=BATCH_BYTES):
     sizes -- this returns the member's name.  (A member that decodes to fewer bytes than its recorded size is also
     named; the stdlib passes it when the CRC-32 of the shorter output matches.)"""
     return _with_decoder(ctx, lambda dec: testzip_with(zip_path, dec, batch_bytes)[0])
+
+
+# ---- strip_zip: inflate, strip and deflate chained on the device -------------------------------------------------
+# Three seams, each an object a CPU stand-in can replace: the decoder (`run_device`: members decoded and left in
+# device memory), the stripper below and the encoder (`submit_device`: a piece gathered from device memory).  What
+# travels between them is a reference, a (device address, length) pair; only those objects look inside one.
+
+SO_SUFFIX = ".so"   # the reference's `find -name "*.so"`
+_S_IFMT, _S_IFLNK = 0o170000, 0o120000
+
+
+class StripFailed(RuntimeError):
+    """A selected member that `strip` refuses: where the reference's `xargs strip` exits 123 and the build stops."""
+
+    def __init__(self, name, why):
+        super().__init__("%s: %s" % (name, why))
+        self.member = name
+
+
+def host_strip(data):
+    """`strip` (the host binary, the reference's own tool) on `data` in a temporary file: the new bytes, or None
+    when strip refuses the file."""
+    fd, path = tempfile.mkstemp(suffix=SO_SUFFIX)
+    try:
+        with os.fdopen(fd, "wb") as f:
+            f.write(data)
+        if subprocess.run(["strip", path], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL).returncode != 0:
+            return None
+        with open(path, "rb") as f:
+            return f.read()
+    finally:
+        os.unlink(path)
+
+
+class GpuStripper:
+    """lb2_strip_device_async / lb2_batch_results over files that already lie in device memory.
+
+    strip(refs): refs are (address, size) with every address a multiple of 16 inside one device buffer (the
+    decoder's); returns [(LB2_ST_* status, (address, size) of the stripped file in the output arena)], valid until
+    the next strip().  fetch(ref) brings a file to the host and upload(data) puts one on the device (until the next
+    strip()): the two directions of the host-strip fallback, counted in uploaded / downloaded.  host_strip is the
+    fallback itself."""
+
+    host_strip = staticmethod(host_strip)
+
+    def __init__(self, ctx):
+        self._ctx, self._out, self._cap, self._extra = ctx, None, 0, []
+        self.uploaded = self.downloaded = 0
+        self._stats = {"plan_ms": 0.0, "compact_ms": 0.0}
+
+    def _release(self):
+        for p in self._extra:
+            self._ctx.dev_free(p)
+        self._extra = []
+
+    def strip(self, refs):
+        self._release()
+        n = len(refs)
+        if not n:
+            return []
+        base = min(a for a, _ in refs)
+        off = (C.c_uint64 * (n + 1))(*[a - base for a, _ in refs], 0)
+        sizes = (C.c_uint64 * n)(*[k for _, k in refs])
+        need = sum(-(-k // 256) * 256 for _, k in refs) + 4096 * n + (1 << 20)
+        out_off, out_sizes, status, st = (C.c_uint64 * (n + 1))(), (C.c_uint64 * n)(), (C.c_int32 * n)(), N.Stats()
+        lib, ctx = self._ctx.lib, self._ctx
+        while True:
+            if need > self._cap:
+                if self._out is not None:
+                    ctx.dev_free(self._out)
+                    self._out, self._cap = None, 0
+                self._out = ctx.dev_alloc(need)
+                self._cap = need
+            ctx.check(lib.lb2_strip_device_async(ctx.h, base, off, sizes, n, self._out, self._cap, 0, None))
+            rc = lib.lb2_batch_results(ctx.h, out_off, out_sizes, status, C.byref(st))
+            if rc == N.LB2_E_CAPACITY and st.out_bytes_needed + (1 << 20) > self._cap:  # re-laid-out files can grow
+                need = st.out_bytes_needed + (1 << 20)
+                continue
+            ctx.check(rc)
+            break
+        self._stats["plan_ms"] += st.plan_ms
+        self._stats["compact_ms"] += st.compact_ms
+        return [(status[i], (self._out + out_off[i], out_sizes[i])) for i in range(n)]
+
+    def fetch(self, ref):
+        addr, n = ref
+        buf = C.create_string_buffer(n)
+        if n:
+            self._ctx.d2h(buf, addr, n)
+        self.downloaded += n
+        return buf.raw
+
+    def upload(self, data):
+        p = self._ctx.dev_alloc(len(data))
+        self._extra.append(p)
+        if data:
+            self._ctx.h2d(p, data, len(data))
+        self.uploaded += len(data)
+        return p, len(data)
+
+    def stats(self):
+        return dict(self._stats)
+
+    def close(self):
+        self._release()
+        if self._out is not None:
+            self._ctx.dev_free(self._out)
+            self._out, self._cap = None, 0
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+def selected_for_strip(zi):
+    """None: the reference's line never sees the member; True: a regular file `find -name "*.so"` hands to strip;
+    False: a matching name that is a directory entry or (by its Unix mode) a symlink, which is left alone."""
+    name = zi.filename[:-1] if zi.is_dir() else zi.filename
+    if not name.rsplit("/", 1)[-1].endswith(SO_SUFFIX):
+        return None
+    return not zi.is_dir() and (zi.external_attr >> 16) & _S_IFMT != _S_IFLNK
+
+
+def _kept(zi):
+    """A copy of a source archive's ZipInfo for the archive being written: no data descriptor (the sizes are known),
+    no zip64 extra field (FileHeader and central_directory make their own)."""
+    out = copy.copy(zi)
+    out.flag_bits &= ~zipfile._MASK_USE_DATA_DESCRIPTOR
+    out.extra = zipfile._strip_extra(zi.extra, (1,))
+    return out
+
+
+def _device_pieces(items, piece, max_segs):
+    """Cut items [(entry index, (address, size))] into pieces as write_zip cuts files: yields ([(entry index,
+    (address, bytes))], flags); a file that does not fit in the rest of a piece leaves a multiple of CHUNK in it."""
+    fill, segs, cont = 0, [], False
+    for idx, (addr, n) in items:
+        pos = 0
+        while True:
+            off = -(-fill // ALIGN) * ALIGN
+            if len(segs) == max_segs or off > piece or (n - pos > piece - off and piece - off < CHUNK):
+                yield segs, N.ZIP_CONTINUES if cont else 0
+                segs, cont, off = [], False, 0
+            want = n - pos if n - pos <= piece - off else (piece - off) // CHUNK * CHUNK
+            segs.append((idx, (addr + pos, want)))
+            fill, pos = off + want, pos + want
+            if pos == n:
+                break
+            yield segs, (N.ZIP_CONTINUES if cont else 0) | N.ZIP_MORE
+            fill, segs, cont = 0, [], True
+    if segs:
+        yield segs, N.ZIP_CONTINUES if cont else 0
+
+
+def strip_with(src_zip, dst_zip, decoder, stripper, encoder, fallback_host_strip=True, tolerate_non_elf=False,
+               batch_bytes=BATCH_BYTES):
+    """strip_zip with the three engines given (GpuUnzipDecoder, GpuStripper, GpuZipEncoder, or stand-ins with the
+    same interfaces)."""
+    src_zip, dst_zip = os.fspath(src_zip), os.fspath(dst_zip)
+    if os.path.realpath(src_zip) == os.path.realpath(dst_zip) or \
+            (os.path.exists(dst_zip) and os.path.samefile(src_zip, dst_zip)):
+        raise ValueError("strip_zip: %r is the archive being read; write the result somewhere else" % dst_zip)
+    piece, max_segs = encoder.piece_bytes, encoder.max_segs
+    if piece < CHUNK:
+        raise ValueError("pieces of %d bytes: at least %d are needed" % (piece, CHUNK))
+    out_dir = os.path.dirname(dst_zip) or "."
+    os.makedirs(out_dir, exist_ok=True)
+    fd, tmp = tempfile.mkstemp(prefix=os.path.basename(dst_zip) + ".", suffix=".tmp", dir=out_dir)
+    try:
+        with os.fdopen(fd, "w+b") as fp, zipfile.ZipFile(src_zip) as zf, open(src_zip, "rb") as src:
+            src.seek(0, os.SEEK_END)
+            archive_bytes = src.tell()
+            entries = [(None, _kept(zi)) for zi in zf.filelist]
+            n = {"selected": 0, "gpu": 0, "fallback": 0, "skipped": 0, "in_bytes": 0, "uploaded": 0, "downloaded": 0}
+
+            def local_body(zi):
+                """the offset of zi's body in src, from its local header"""
+                src.seek(zi.header_offset)
+                fh = src.read(zipfile.sizeFileHeader)
+                if len(fh) != zipfile.sizeFileHeader or fh[:4] != zipfile.stringFileHeader:
+                    raise zipfile.BadZipFile("Bad magic number for file header of %r" % zi.filename)
+                fh = struct.unpack(zipfile.structFileHeader, fh)
+                return zi.header_offset + zipfile.sizeFileHeader + fh[zipfile._FH_FILENAME_LENGTH] + \
+                    fh[zipfile._FH_EXTRA_FIELD_LENGTH]
+
+            origin = {id(out): zi for (_, out), zi in zip(entries, zf.filelist)}  # entry written -> the source's
+
+            def copy_member(out):
+                zi = origin[id(out)]
+                start = local_body(zi)
+                fp.write(out.FileHeader())
+                src.seek(start)
+                left = zi.compress_size
+                while left:
+                    block = src.read(min(left, 1 << 20))
+                    if not block:
+                        raise zipfile.BadZipFile("%s ends inside the body of %r" % (src_zip, zi.filename))
+                    fp.write(block)
+                    left -= len(block)
+
+            w = _ContainerWriter(fp, entries, copy=copy_member)
+            in_flight = []
+
+            def collect():
+                body, res = encoder.collect()
+                n["downloaded"] += len(body)
+                for (idx, (_, nbytes)), (off, k, crc, ended) in zip(in_flight.pop(0), res):
+                    w.part(idx, body[off:off + k], crc, ended, nbytes)
+
+            def host_path(idx, zi, data):
+                """the stripped bytes of a member the device did not strip, on the device; None: keep the member"""
+                new = stripper.host_strip(data) if fallback_host_strip else None
+                if new is None:
+                    if tolerate_non_elf and data[:4] != b"\x7fELF":
+                        n["skipped"] += 1
+                        return None
+                    raise StripFailed(zi.filename, "strip refuses this file (the reference's xargs exits 123)"
+                                      if fallback_host_strip else "not stripped on the GPU, and the host strip is off")
+                n["fallback"] += 1
+                return stripper.upload(new)
+
+            def run(batch):
+                """batch: [(entry index, source ZipInfo)] of selected members, in archive order"""
+                view = decoder.buffer(sum(zi.compress_size for _, zi in batch))
+                members, taken, fill = [], [], 0
+                for idx, zi in batch:
+                    if not _gpu_member(zi):
+                        continue
+                    src.seek(zi.header_offset)
+                    head = src.read(zipfile.sizeFileHeader)
+                    if len(head) == zipfile.sizeFileHeader:
+                        fh = struct.unpack(zipfile.structFileHeader, head)
+                        head += src.read(fh[zipfile._FH_FILENAME_LENGTH] + fh[zipfile._FH_EXTRA_FIELD_LENGTH])
+                    b = _body(zf, zi, head, zi.header_offset, archive_bytes)
+                    if b is None or b[0] != len(head):
+                        continue                       # the stdlib's own code reads it, and raises what it raises
+                    if b[1] < 0 or _read_into(src, view[fill:fill + zi.compress_size]) != zi.compress_size:
+                        raise BadZipMember(zi.filename, "The archive ends inside the body")
+                    members.append((fill, zi.compress_size, zi.file_size, zi.CRC, zi.compress_type))
+                    taken.append(idx)
+                    fill += zi.compress_size
+                decoded = {}
+                try:
+                    if taken:
+                        decoded = dict(zip(taken, decoder.run_device(fill, members)))
+                        n["uploaded"] += fill
+                except DeviceTooSmall:
+                    if len(taken) > 1:
+                        run(batch[:len(batch) // 2])
+                        run(batch[len(batch) // 2:])
+                        return
+                    # a member that does not fit on the device alone: read by the stdlib, stripped on the host
+                for idx, zi in batch:
+                    status = decoded.get(idx, (UNZIP_OK, None))[0]
+                    if status != UNZIP_OK:
+                        raise BadZipMember(zi.filename, {UNZIP_BAD_DATA: "Invalid DEFLATE data", UNZIP_BAD_CRC: "Bad CRC-32",
+                                                         UNZIP_WRONG_SIZE: "Wrong uncompressed size"}[status])
+                on_device = [(idx, zi) for idx, zi in batch if idx in decoded]
+                stripped = dict(zip([idx for idx, _ in on_device],
+                                    stripper.strip([decoded[idx][1] for idx, _ in on_device])))
+                items = []
+                for idx, zi in batch:
+                    if idx in stripped and stripped[idx][0] == N.ST_OK:
+                        ref = stripped[idx][1]
+                        n["gpu"] += 1
+                    elif idx in stripped and stripped[idx][0] == N.ST_NOT_ELF and tolerate_non_elf:
+                        n["skipped"] += 1
+                        continue
+                    else:
+                        ref = host_path(idx, zi, stripper.fetch(decoded[idx][1]) if idx in decoded else zf.read(zi))
+                        if ref is None:
+                            continue
+                    entries[idx][1].file_size = ref[1]   # the writer's zip64 choice is made from it
+                    n["in_bytes"] += zi.file_size
+                    items.append((idx, ref))
+                for segs, flags in _device_pieces(items, piece, max_segs):
+                    encoder.submit_device([ref for _, ref in segs], flags)
+                    in_flight.append(segs)
+                    if len(in_flight) == 2:
+                        collect()
+                while in_flight:  # the next batch replaces the buffers these pieces read
+                    collect()
+
+            batch, cost = [], 0
+            for idx, zi in enumerate(zf.filelist):
+                sel = selected_for_strip(zi)
+                if not sel:
+                    n["skipped"] += sel is False
+                    continue
+                n["selected"] += 1
+                c = zi.compress_size + 4 * zi.file_size + 1024
+                if batch and cost + c > batch_bytes:
+                    run(batch)
+                    batch, cost = [], 0
+                batch.append((idx, zi))
+                cost += c
+            if batch:
+                run(batch)
+            w.finish(zf.comment)
+            zip_bytes = fp.tell()
+        os.chmod(tmp, 0o666 & ~_umask())
+        os.replace(tmp, dst_zip)
+    except BaseException:
+        os.unlink(tmp)
+        raise
+    st = {"members": len(entries), "selected": n["selected"], "gpu": n["gpu"], "fallback": n["fallback"],
+          "skipped": n["skipped"], "in_bytes": n["in_bytes"], "out_bytes": w.in_bytes, "deflated_bytes": w.out_bytes,
+          "src_zip_bytes": archive_bytes, "zip_bytes": zip_bytes,
+          "uploaded_bytes": n["uploaded"] + stripper.uploaded, "downloaded_bytes": n["downloaded"] + stripper.downloaded,
+          "unzip": decoder.stats(), "strip": stripper.stats(), "deflate": encoder.stats()}
+    st["kernel_ms"] = st["unzip"].get("kernel_ms", 0.0) + sum(st["strip"].values()) + st["deflate"].get("kernel_ms", 0.0)
+    return st
+
+
+def _umask():
+    mask = os.umask(0)
+    os.umask(mask)
+    return mask
+
+
+def strip_zip(src_zip, dst_zip, ctx=None, compresslevel=None, fallback_host_strip=True, tolerate_non_elf=False,
+              batch_bytes=BATCH_BYTES, piece_bytes=PIECE_BYTES):
+    """Write `dst_zip` with the members of `src_zip`, in their order, every `*.so` member stripped: the archive that
+    `ZipFile(src_zip).extractall(d)`, the reference's `find d/ -name "*.so" | xargs strip` and a zip of `d` lead to,
+    without the tree.  src_zip is only read; dst_zip appears under its name when it is complete, and not at all when
+    the call raises; dst_zip == src_zip raises ValueError.
+
+    Selected: regular-file members whose basename ends in ".so" (directory entries and members whose Unix mode says
+    symlink are counted as skipped).  In batches bounded by device memory their bodies are uploaded, inflated and
+    CRC-checked (lb2_unzip_run), stripped where they lie (lb2_strip_device_async) and deflated from the stripped arena
+    (lb2_zip_submit_device), so only compressed bytes cross the bus; each becomes a ZIP_DEFLATED member with its new
+    CRC-32 and sizes.  Every other member's body, method, CRC-32, sizes, name, time, attributes, extra field and
+    comment are copied as they are under a fresh local header (no data descriptor; zip64 fields regenerated); the
+    archive comment is kept, bytes in front of the first member are not.
+
+    An ELF the planner refuses is fetched, stripped by the host `strip` and uploaded again (fallback_host_strip), as
+    in strip_tree; so is a selected member the GPU reader does not take (encrypted, bzip2 ...: the stdlib reads it
+    and raises what it raises).  A member `strip` refuses raises StripFailed -- the reference's xargs exits 123 --
+    unless it is not an ELF and tolerate_non_elf keeps it as it is.  A member that does not read back raises
+    BadZipMember.  compresslevel: None or 9, as zip_tree.
+
+    Returns a stats dict: members, selected, gpu, fallback, skipped; in_bytes / out_bytes (the stripped members
+    before and after) and deflated_bytes (their new bodies); src_zip_bytes, zip_bytes; uploaded_bytes,
+    downloaded_bytes (everything that crossed the bus for member data); unzip, strip (plan_ms, compact_ms) and
+    deflate (the three engines' stats) and kernel_ms, their kernel times summed.  There is no CPU path: without a
+    GPU this raises."""
+    from .tarball import _default_context
+    N.deflate_flags(compresslevel)
+    own = False
+    if ctx is None:
+        ctx, own = _default_context()
+    try:
+        with GpuUnzipDecoder(ctx) as dec, GpuStripper(ctx) as stripper, \
+                GpuZipEncoder(ctx, piece_bytes, compresslevel=compresslevel, host_buffers=False) as enc:
+            return strip_with(src_zip, dst_zip, dec, stripper, enc, fallback_host_strip, tolerate_non_elf, batch_bytes)
+    finally:
+        if own:
+            ctx.close()
+
+
+def main(argv=None):
+    """python -m lambdipy_b200.zipfile_gpu strip SRC DST [--level 9]"""
+    import argparse
+    from . import patch, project_build
+    ap = argparse.ArgumentParser(prog="python -m lambdipy_b200.zipfile_gpu")
+    sub = ap.add_subparsers(dest="command", required=True)
+    sp = sub.add_parser("strip", help="strip the *.so members of SRC on the GPU and write the result to DST")
+    sp.add_argument("src")
+    sp.add_argument("dst")
+    sp.add_argument("--level", type=int, choices=[9], default=None, help="9: the optimal parse (smaller, slower)")
+    args = ap.parse_args(argv)
+    st = strip_zip(args.src, args.dst, compresslevel=args.level)
+    with zipfile.ZipFile(args.dst) as zf:
+        unzipped = sum(zi.file_size for zi in zf.filelist)
+    print("Bundle zip: %s, %.1f MB = %.0f %% of the 50 MB direct-upload limit; unzipped %.1f MB = %.0f %% of 250 MB; "
+          "%d shared objects stripped (%d via host strip), %.1f MB -> %.1f MB"
+          % (args.dst, st["zip_bytes"] / 1e6, 100.0 * st["zip_bytes"] / patch.LAMBDA_ZIPPED_LIMIT, unzipped / 1e6,
+             100.0 * unzipped / project_build.LAMBDA_UNZIPPED_LIMIT, st["gpu"] + st["fallback"], st["fallback"],
+             st["in_bytes"] / 1e6, st["out_bytes"] / 1e6))
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())
