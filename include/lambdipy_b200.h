@@ -126,6 +126,8 @@ void lb2_pinned_free(lb2_ctx *ctx, void *p);
 int lb2_memcpy_h2d(lb2_ctx *ctx, void *d_dst, const void *h_src, uint64_t bytes);
 int lb2_memcpy_d2h(lb2_ctx *ctx, void *h_dst, const void *d_src, uint64_t bytes);
 int lb2_memset_d(lb2_ctx *ctx, void *d_dst, int value, uint64_t bytes);
+/* device to device; returns when the copy is done, as the two above */
+int lb2_memcpy_d2d(lb2_ctx *ctx, void *d_dst, const void *d_src, uint64_t bytes);
 
 /* ---- strip a batch resident in HBM ------------------------------------------------------ */
 /* d_in: input arena; file f occupies [h_in_off[f], h_in_off[f+1]) minus padding -- offsets must be
@@ -257,6 +259,15 @@ int lb2_gzip_collect(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n
 /* writes the final block (2 bytes); *crc32 / *isize (full length; gzip stores it mod 2^32) for the trailer */
 int lb2_gzip_finish(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n, uint32_t *crc32, uint64_t *isize,
                     lb2_gzip_stats *stats);
+/* A piece whose bytes are already in device memory, which is how tarball.strip_tarball strips the shared objects inside
+ * a .tar.gz without the tar stream leaving the device.  The piece is src[0].len + ... + src[n_segs - 1].len bytes: the
+ * segments (lb2_zip_source, of any alignment) back to back, with no padding.  A gather kernel on the writer's stream
+ * lays them out in the piece buffer; from there the piece is what lb2_gzip_submit makes of the concatenation -- the
+ * same chunks, history, CRC-32, ISIZE, bytes out and LB2_E_STATE cases (stats.h2d_ms then times the gather).
+ * n_segs may be 0 (an empty piece).  The caller guarantees that the sources are complete when this is called and
+ * leaves them unchanged until the piece is collected. */
+struct lb2_zip_source;
+int lb2_gzip_submit_device(lb2_gzip *g, const struct lb2_zip_source *src, uint32_t n_segs);
 void lb2_gzip_destroy(lb2_gzip *g);
 
 /* ---- zip writer: one raw DEFLATE stream + CRC-32 per file, many files per piece ------------------ */
@@ -346,6 +357,9 @@ int lb2_inflate_create(lb2_ctx *ctx, uint32_t flags /* 0 */, lb2_inflate **d);
 int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_n, lb2_inflate_stats *stats);
 /* copy the decoded bytes of the last successful run to h_out (cap >= *out_n) */
 int lb2_inflate_read(lb2_inflate *d, void *h_out, uint64_t cap);
+/* The device buffer lb2_inflate_read would copy from: *n bytes at *d_out (NULL when *n is 0), 256-byte aligned.  Valid
+ * until the next lb2_inflate_run or lb2_inflate_destroy.  LB2_E_STATE without a successful run. */
+int lb2_inflate_device_output(lb2_inflate *d, const void **d_out, uint64_t *n);
 void lb2_inflate_destroy(lb2_inflate *d);
 
 /* ---- zip reader: every member of a zip decoded and checked on the GPU in one batch ------------------ */
@@ -406,6 +420,32 @@ int lb2_unzip_read(lb2_unzip *u, void *h_out, uint64_t cap);
  * without a successful run. */
 int lb2_unzip_device_output(lb2_unzip *u, const void **d_out, uint64_t *n);
 void lb2_unzip_destroy(lb2_unzip *u);
+
+/* ---- tar index: the bytes tarfile reads to list the members of a tar stream in device memory ---------------- */
+/* One warp walks the headers of d_tar[0 .. n) (16-byte aligned) the way Python 3.12's tarfile lists members (USTAR,
+ * GNU, PAX and v7 headers; GNU long names, pax records of up to 1 MiB, GNU old-sparse extension blocks) and gathers
+ * every range that listing reads: each header block, the byte in front of it (TarFile.next reads it to check that the
+ * previous member's data exists), the extended headers' data, and the block where the walk stopped (an all-zero
+ * block, a header tarfile refuses, the end of the data, or something the walk does not follow).  ranges[0 .. *n_ranges)
+ * are sorted, do not touch each other, and their bytes are in h_bytes[0 .. *n_bytes) back to back.  A caller that
+ * lists the members with tarfile from these bytes reads nothing else on the archives people have, and fetches
+ * whatever else it reads.
+ * LB2_E_CAPACITY when max_ranges or bytes_cap is too small: *n_ranges / *n_bytes say what is needed, stats is filled. */
+typedef struct lb2_tar_range {
+  uint64_t off, len;
+} lb2_tar_range;
+#define LB2_TAR_STOP_ZERO 1          /* an all-zero block: the end-of-archive marker                                  */
+#define LB2_TAR_STOP_BAD_HEADER 2    /* a bad checksum or a number field tarfile refuses                              */
+#define LB2_TAR_STOP_END 3           /* the end of the data, inside or right at a header                              */
+#define LB2_TAR_STOP_UNSUPPORTED 4   /* an extended header over 1 MiB, pax records the walk does not follow          */
+typedef struct lb2_tar_index_stats {
+  uint64_t n_members;      /* member headers walked (extended headers not counted)                                  */
+  uint64_t stop_offset;    /* the offset of the block the walk stopped at                                           */
+  uint32_t stop_reason;    /* LB2_TAR_STOP_*                                                                        */
+  float kernel_ms;         /* the walk kernel (CUDA events)                                                         */
+} lb2_tar_index_stats;
+int lb2_tar_index(lb2_ctx *ctx, const void *d_tar, uint64_t n, lb2_tar_range *ranges, uint32_t max_ranges,
+                  uint32_t *n_ranges, void *h_bytes, uint64_t bytes_cap, uint64_t *n_bytes, lb2_tar_index_stats *stats);
 
 #ifdef __cplusplus
 }

@@ -8,6 +8,8 @@ Public surface:
     gzip_tarball(src_paths, tarball_path)       tar.gz of a package tree, DEFLATE on the GPU
     tarball.create_compressed_tarball           mirror of PackageBuild.create_compressed_tarball
     gunzip(path)                                decompressed bytes of a gzip file, DEFLATE decoded on the GPU
+    strip_tarball(src, dst)                     a .tar.gz with its shared objects stripped, inflated, stripped
+                                                and deflated on the GPU without unpacking it
     tarball.prepare_tarfile                     mirror of the reference's prepare_tarfile
     zip_tree(root_dir, zip_path)                the Lambda deployment zip of a tree (shutil.make_archive's
                                                 archive), every member's DEFLATE body compressed on the GPU
@@ -23,7 +25,7 @@ def __getattr__(name):
     if name in ("strip_tree", "strip_buffers"):
         from . import strip
         return getattr(strip, name)
-    if name in ("gzip_tarball", "gunzip"):
+    if name in ("gzip_tarball", "gunzip", "strip_tarball"):
         from . import tarball
         return getattr(tarball, name)
     if name in ("zip_tree", "extract_zip", "testzip"):

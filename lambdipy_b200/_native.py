@@ -29,7 +29,9 @@ EXPORTS = [
     "lb2_zip_create", "lb2_zip_submit", "lb2_zip_collect", "lb2_zip_destroy",
     "lb2_unzip_create", "lb2_unzip_run", "lb2_unzip_read", "lb2_unzip_destroy",
     "lb2_zip_submit_device", "lb2_unzip_device_output",
+    "lb2_inflate_device_output", "lb2_memcpy_d2d", "lb2_gzip_submit_device", "lb2_tar_index",
 ]
+TAR_STOP_ZERO, TAR_STOP_BAD_HEADER, TAR_STOP_END, TAR_STOP_UNSUPPORTED = 1, 2, 3, 4
 ZIP_CONTINUES, ZIP_MORE = 1, 2
 DEFLATE_BEST = 1  # LB2_DEFLATE_BEST
 
@@ -131,6 +133,18 @@ class UnzipStats(C.Structure):
         ("h2d_ms", C.c_float), ("copy_ms", C.c_float), ("small_ms", C.c_float), ("find_ms", C.c_float),
         ("count_ms", C.c_float), ("decode_ms", C.c_float), ("resolve_ms", C.c_float), ("crc_ms", C.c_float),
     ]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class TarRange(C.Structure):
+    _fields_ = [("off", C.c_uint64), ("len", C.c_uint64)]
+
+
+class TarIndexStats(C.Structure):
+    _fields_ = [("n_members", C.c_uint64), ("stop_offset", C.c_uint64), ("stop_reason", C.c_uint32),
+                ("kernel_ms", C.c_float)]
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
@@ -249,6 +263,15 @@ def load():
     lib.lb2_unzip_device_output.restype = C.c_int
     lib.lb2_unzip_destroy.argtypes = [vp]
     lib.lb2_unzip_destroy.restype = None
+    lib.lb2_inflate_device_output.argtypes = [vp, C.POINTER(vp), u64p]
+    lib.lb2_inflate_device_output.restype = C.c_int
+    lib.lb2_memcpy_d2d.argtypes = [vp, vp, vp, C.c_uint64]
+    lib.lb2_memcpy_d2d.restype = C.c_int
+    lib.lb2_gzip_submit_device.argtypes = [vp, C.POINTER(ZipSource), C.c_uint32]
+    lib.lb2_gzip_submit_device.restype = C.c_int
+    lib.lb2_tar_index.argtypes = [vp, vp, C.c_uint64, C.POINTER(TarRange), C.c_uint32, C.POINTER(C.c_uint32), vp,
+                                  C.c_uint64, u64p, C.POINTER(TarIndexStats)]
+    lib.lb2_tar_index.restype = C.c_int
     _lib = lib
     return lib
 
@@ -320,3 +343,6 @@ class Context:
 
     def d2h(self, h, d, n):
         self.check(self.lib.lb2_memcpy_d2h(self.h, h, d, n))
+
+    def d2d(self, dst, src, n):
+        self.check(self.lib.lb2_memcpy_d2d(self.h, dst, src, n))

@@ -312,6 +312,14 @@ void lb2_pinned_free(lb2_ctx *, void *p) { if (p) cudaFreeHost(p); }
 int lb2_memcpy_h2d(lb2_ctx *ctx, void *d, const void *h, uint64_t n) { CK(cudaMemcpy(d, h, n, cudaMemcpyHostToDevice)); return LB2_OK; }
 int lb2_memcpy_d2h(lb2_ctx *ctx, void *h, const void *d, uint64_t n) { CK(cudaMemcpy(h, d, n, cudaMemcpyDeviceToHost)); return LB2_OK; }
 int lb2_memset_d(lb2_ctx *ctx, void *d, int v, uint64_t n) { CK(cudaMemset(d, v, n)); return LB2_OK; }
+int lb2_memcpy_d2d(lb2_ctx *ctx, void *d, const void *s, uint64_t n) {
+  if (!ctx) return LB2_E_ARG;
+  if ((!d || !s) && n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if (!n) return LB2_OK;
+  CK(cudaMemcpy(d, s, n, cudaMemcpyDeviceToDevice));
+  CK(cudaStreamSynchronize(0));  // a device-to-device cudaMemcpy may return before the copy is done
+  return LB2_OK;
+}
 
 int lb2_strip_device_async(lb2_ctx *ctx, const void *d_in, const uint64_t *h_in_off, const uint64_t *h_in_sizes,
                            uint32_t n_files, void *d_out, uint64_t out_capacity, uint32_t flags, void *stream) {
@@ -595,10 +603,13 @@ static void gz_destroy(GzWriter *g) {
 }
 
 // Enqueue one piece of n bytes holding n_segs segments [seg_off[i], seg_off[i] + seg_len[i]) (validated by the
-// caller).  The piece is uploaded from h_in, or, when d_src is given, gathered on the device: segment i is seg_len[i]
-// bytes at d_src[i].d_ptr.  cont: segment 0 continues the open stream / file; ends: segment i's file ends in this piece.
-static int gz_submit(GzWriter *g, const void *h_in, const lb2_zip_source *d_src, uint64_t n, const uint64_t *seg_off,
-                     const uint64_t *seg_len, uint32_t n_segs, bool cont, bool last_ends) {
+// caller).  The piece is uploaded from h_in, or, when d_src is given, gathered on the device: source j is d_src[j].len
+// bytes at d_src[j].d_ptr, laid out at src_dst[j] of the piece and, with pad, followed by zeros up to the next multiple
+// of 16 (the zip writer's segments: one source each).  cont: segment 0 continues the open stream / file; ends: segment
+// i's file ends in this piece.
+static int gz_submit(GzWriter *g, const void *h_in, const lb2_zip_source *d_src, uint32_t n_src, const uint64_t *src_dst,
+                     bool pad, uint64_t n, const uint64_t *seg_off, const uint64_t *seg_len, uint32_t n_segs, bool cont,
+                     bool last_ends) {
   lb2_ctx *ctx = g->ctx;
   CK(cudaSetDevice(ctx->device));
   GzSlot &s = g->slot[(g->head + g->count) & 1];
@@ -609,7 +620,7 @@ static int gz_submit(GzWriter *g, const void *h_in, const lb2_zip_source *d_src,
   if (rc) return rc;
   uint64_t n_tiles = 0;
   if (d_src) {
-    for (uint32_t i = 0; i < n_segs; i++) n_tiles += (seg_len[i] + GZ_GATHER_TILE - 1) / GZ_GATHER_TILE;
+    for (uint32_t i = 0; i < n_src; i++) n_tiles += (d_src[i].len + GZ_GATHER_TILE - 1) / GZ_GATHER_TILE;
     if (n_tiles > s.cap_gat) {
       const uint64_t t = std::max(n_tiles, 2 * s.cap_gat);
       cudaFree(s.d_gat);
@@ -621,12 +632,12 @@ static int gz_submit(GzWriter *g, const void *h_in, const lb2_zip_source *d_src,
       s.cap_gat = t;
     }
     GzGatherTile *tile = s.h_gat;
-    for (uint32_t i = 0; i < n_segs; i++)
-      for (uint64_t p = 0; p < seg_len[i]; p += GZ_GATHER_TILE) {
-        const uint32_t len = (uint32_t)std::min<uint64_t>(GZ_GATHER_TILE, seg_len[i] - p);
-        const uint64_t end = seg_off[i] + p + len;
-        *tile++ = GzGatherTile{static_cast<const uint8_t *>(d_src[i].d_ptr) + p, seg_off[i] + p, len,
-                               p + len == seg_len[i] ? (uint32_t)(-end & 15) : 0u};
+    for (uint32_t i = 0; i < n_src; i++)
+      for (uint64_t p = 0; p < d_src[i].len; p += GZ_GATHER_TILE) {
+        const uint32_t len = (uint32_t)std::min<uint64_t>(GZ_GATHER_TILE, d_src[i].len - p);
+        const uint64_t end = src_dst[i] + p + len;
+        *tile++ = GzGatherTile{static_cast<const uint8_t *>(d_src[i].d_ptr) + p, src_dst[i] + p, len,
+                               pad && p + len == d_src[i].len ? (uint32_t)(-end & 15) : 0u};
       }
   }
   GzChunk *chunks = reinterpret_cast<GzChunk *>(s.h_tab);
@@ -762,7 +773,30 @@ int lb2_gzip_submit(lb2_gzip *g, const void *h_in, uint64_t n) {
   }
   // the piece is one segment of the stream, which continues from the previous piece and stays open
   const uint64_t off = 0;
-  return gz_submit(g, h_in, nullptr, n, &off, &n, 1, true, false);
+  return gz_submit(g, h_in, nullptr, 0, nullptr, false, n, &off, &n, 1, true, false);
+}
+
+int lb2_gzip_submit_device(lb2_gzip *g, const lb2_zip_source *src, uint32_t n_segs) {
+  if (!g) return LB2_E_ARG;
+  lb2_ctx *ctx = g->ctx;
+  if (!src && n_segs) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if (g->finished) { ctx->err = "lb2_gzip_submit_device after lb2_gzip_finish"; return LB2_E_STATE; }
+  if (g->count >= 2) { ctx->err = "two pieces already in flight: collect one with lb2_gzip_collect first"; return LB2_E_STATE; }
+  std::vector<uint64_t> dst(n_segs);
+  uint64_t n = 0;  // the piece: the sources back to back
+  for (uint32_t i = 0; i < n_segs; i++) {
+    if (!src[i].d_ptr && src[i].len) { ctx->err = "segment " + std::to_string(i) + ": NULL source"; return LB2_E_ARG; }
+    dst[i] = n;
+    if (src[i].len > (uint64_t)UINT32_MAX * GZ_CHUNK / 2 - n) { ctx->err = "piece too large"; return LB2_E_ARG; }
+    n += src[i].len;
+  }
+  if (!n) {
+    g->slot[(g->head + g->count) & 1].n_segs = 0;
+    g->count++;
+    return LB2_OK;
+  }
+  const uint64_t off = 0;
+  return gz_submit(g, nullptr, src, n_segs, dst.data(), false, n, &off, &n, 1, true, false);
 }
 
 int lb2_gzip_collect(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n) {
@@ -842,7 +876,7 @@ int lb2_zip_submit(lb2_zip *z, const void *h_in, uint64_t n, const uint64_t *seg
     }
     end = seg_off[i] + seg_len[i];
   }
-  return gz_submit(z, h_in, nullptr, n, seg_off, seg_len, n_segs, cont, !(flags & LB2_ZIP_MORE));
+  return gz_submit(z, h_in, nullptr, 0, nullptr, false, n, seg_off, seg_len, n_segs, cont, !(flags & LB2_ZIP_MORE));
 }
 
 int lb2_zip_submit_device(lb2_zip *z, const lb2_zip_source *src, uint32_t n_segs, uint32_t flags) {
@@ -860,7 +894,8 @@ int lb2_zip_submit_device(lb2_zip *z, const lb2_zip_source *src, uint32_t n_segs
     if (len[i] > (uint64_t)UINT32_MAX * GZ_CHUNK / 2 - off[i]) { ctx->err = "piece too large"; return LB2_E_ARG; }
     n = off[i] + len[i];
   }
-  return gz_submit(z, nullptr, src, n, off.data(), len.data(), n_segs, flags & LB2_ZIP_CONTINUES, !(flags & LB2_ZIP_MORE));
+  return gz_submit(z, nullptr, src, n_segs, off.data(), true, n, off.data(), len.data(), n_segs, flags & LB2_ZIP_CONTINUES,
+                   !(flags & LB2_ZIP_MORE));
 }
 
 int lb2_zip_collect(lb2_zip *z, void *h_out, uint64_t out_cap, uint64_t *out_n, lb2_zip_segment *segs, lb2_gzip_stats *stats) {
@@ -1069,6 +1104,16 @@ int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_
   d->out_n = total;
   d->have = true;
   *out_n = total;
+  return LB2_OK;
+}
+
+int lb2_inflate_device_output(lb2_inflate *d, const void **d_out, uint64_t *n) {
+  if (!d) return LB2_E_ARG;
+  lb2_ctx *ctx = d->ctx;
+  if (!d_out || !n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if (!d->have) { ctx->err = "lb2_inflate_device_output: no decoded stream (lb2_inflate_run failed or was not called)"; return LB2_E_STATE; }
+  *d_out = d->out_n ? d->d_out : nullptr;
+  *n = d->out_n;
   return LB2_OK;
 }
 
@@ -1352,6 +1397,57 @@ int lb2_unzip_read(lb2_unzip *u, void *h_out, uint64_t cap) {
   if (!h_out && u->out_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
   CK(cudaSetDevice(ctx->device));
   if (u->out_n) CK(cudaMemcpy(h_out, u->d_out, u->out_n, cudaMemcpyDeviceToHost));
+  return LB2_OK;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------- tar index
+// The walk kernel (tar.cu) on the context's stream; ranges and bytes land in one scratch allocation of the call.
+#include "tar_walk.cuh"
+static_assert(sizeof(lb2_tar_range) == sizeof(tarw::Range), "the walk kernel writes lb2_tar_range records");
+
+extern "C" {
+
+int lb2_tar_index(lb2_ctx *ctx, const void *d_tar, uint64_t n, lb2_tar_range *ranges, uint32_t max_ranges, uint32_t *n_ranges,
+                  void *h_bytes, uint64_t bytes_cap, uint64_t *n_bytes, lb2_tar_index_stats *stats) {
+  if (!ctx) return LB2_E_ARG;
+  if ((!d_tar && n) || !n_ranges || !n_bytes || (!ranges && max_ranges) || (!h_bytes && bytes_cap)) {
+    ctx->err = "NULL argument";
+    return LB2_E_ARG;
+  }
+  if (reinterpret_cast<uintptr_t>(d_tar) & 15) { ctx->err = "lb2_tar_index: d_tar must be 16-byte aligned"; return LB2_E_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  const uint64_t r_bytes = (uint64_t)max_ranges * sizeof(lb2_tar_range);
+  uint8_t *d_ws = nullptr;
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  TarWalkOut out{};
+  float ms = 0;
+  cudaError_t e = cudaMalloc(&d_ws, sizeof(TarWalkOut) + r_bytes + bytes_cap);
+  if (e == cudaSuccess) e = cudaEventCreate(&ev[0]);
+  if (e == cudaSuccess) e = cudaEventCreate(&ev[1]);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[0], ctx->stream);
+  if (e == cudaSuccess) {
+    launch_tar_walk(static_cast<const uint8_t *>(d_tar), n, d_ws + sizeof(TarWalkOut), max_ranges,
+                    d_ws + sizeof(TarWalkOut) + r_bytes, bytes_cap, reinterpret_cast<TarWalkOut *>(d_ws), ctx->stream);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaEventRecord(ev[1], ctx->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&out, d_ws, sizeof out, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ev[0], ev[1]);
+  const bool fits = out.n_ranges <= max_ranges && out.n_bytes <= bytes_cap;
+  if (e == cudaSuccess && fits && out.n_ranges)
+    e = cudaMemcpy(ranges, d_ws + sizeof(TarWalkOut), out.n_ranges * sizeof(lb2_tar_range), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess && fits && out.n_bytes)
+    e = cudaMemcpy(h_bytes, d_ws + sizeof(TarWalkOut) + r_bytes, out.n_bytes, cudaMemcpyDeviceToHost);
+  cudaFree(d_ws);
+  for (auto &v : ev) if (v) cudaEventDestroy(v);
+  if (e != cudaSuccess) { ctx->err = std::string("lb2_tar_index: ") + cudaGetErrorString(e); return LB2_E_CUDA; }
+  *n_ranges = out.n_ranges > UINT32_MAX ? UINT32_MAX : (uint32_t)out.n_ranges;
+  *n_bytes = out.n_bytes;
+  if (stats) *stats = lb2_tar_index_stats{out.members, out.stop_off, out.reason, ms};
+  if (!fits) { ctx->err = "lb2_tar_index: ranges or bytes exceed the capacity given (*n_ranges, *n_bytes needed)"; return LB2_E_CAPACITY; }
   return LB2_OK;
 }
 
