@@ -268,6 +268,13 @@ int lb2_gzip_finish(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n,
  * leaves them unchanged until the piece is collected. */
 struct lb2_zip_source;
 int lb2_gzip_submit_device(lb2_gzip *g, const struct lb2_zip_source *src, uint32_t n_segs);
+/* The compressed size of every 64 KB chunk of the piece collected last, in stream order: sizes[0 .. *n_chunks), which
+ * sum to that collect's *out_n (an empty piece has none).  Chunk i of a piece of n bytes holds its bytes
+ * [64 KB * i, min(n, 64 KB * (i + 1))), and every chunk ends byte-aligned with an empty stored block, so the next
+ * one starts a block at a known byte: what a seek table records (seek_table.py).  Call it after lb2_gzip_collect and
+ * before the next submit reuses that piece's slot (LB2_E_STATE otherwise); LB2_E_CAPACITY when cap is too small
+ * (*n_chunks says how many).  The final block that lb2_gzip_finish writes is not part of any chunk. */
+int lb2_gzip_chunk_sizes(lb2_gzip *g, uint32_t *sizes, uint32_t cap, uint32_t *n_chunks);
 void lb2_gzip_destroy(lb2_gzip *g);
 
 /* ---- zip writer: one raw DEFLATE stream + CRC-32 per file, many files per piece ------------------ */
@@ -326,6 +333,10 @@ typedef struct lb2_zip_source {
   uint64_t len;                /* bytes; 0 for an empty file (d_ptr may then be NULL)                       */
 } lb2_zip_source;
 int lb2_zip_submit_device(lb2_zip *z, const lb2_zip_source *src, uint32_t n_segs, uint32_t flags);
+/* lb2_gzip_chunk_sizes for the zip writer: the compressed size of every 64 KB chunk of the piece collected last, in
+ * segment order (a segment of n bytes has max(1, ceil(n / 64 KB)) chunks, cut at multiples of 64 KB of the segment;
+ * the last chunk of a file that ended includes its final block 03 00).  Each segment's sizes sum to its out_len. */
+int lb2_zip_chunk_sizes(lb2_zip *z, uint32_t *sizes, uint32_t cap, uint32_t *n_chunks);
 void lb2_zip_destroy(lb2_zip *z);
 
 /* ---- gzip reader: raw DEFLATE (RFC 1951) decoded on the GPU ----------------------------------- */
@@ -360,6 +371,22 @@ int lb2_inflate_read(lb2_inflate *d, void *h_out, uint64_t cap);
 /* The device buffer lb2_inflate_read would copy from: *n bytes at *d_out (NULL when *n is 0), 256-byte aligned.  Valid
  * until the next lb2_inflate_run or lb2_inflate_destroy.  LB2_E_STATE without a successful run. */
 int lb2_inflate_device_output(lb2_inflate *d, const void **d_out, uint64_t *n);
+/* A stream with a seek table (seek_table.py): spans[i] is the compressed and the decoded length of a run of the
+ * stream, in order from its first byte; every run after the first starts with a block header at its first byte.  Each
+ * run is decoded once, by one thread, from its known start into its known output range (lb2_inflate_table_decode_
+ * kernel): no candidate search, no count rounds.  The table is outside input.  It is refused without a launch when an
+ * entry is 0, decodes to more than 1032 bytes per compressed byte or the runs pass n; it is refused after the decode
+ * unless every run decoded exactly its length and ended at the block header the next run starts at, and only the last
+ * run decoded the final block, ending with the table's last byte.  An accepted table therefore gives exactly the
+ * stream's DEFLATE decode; a refused one is followed by the search of lb2_inflate_run on the same stream.  Either way
+ * the bytes, CRC-32, return code and stats.in_bytes are what lb2_inflate_run gives: a lying table costs time, never a
+ * different result.  *n_table = 1 when the stream was decoded from the table (stats: 0 find and count rounds,
+ * n_spans = the entries), *n_refused = 1 when a table was given and refused (both may be NULL). */
+typedef struct lb2_inflate_span {
+  uint64_t in_len, out_len;       /* compressed bytes, decoded bytes                                              */
+} lb2_inflate_span;
+int lb2_inflate_run_table(lb2_inflate *d, const void *h_in, uint64_t n, const lb2_inflate_span *spans, uint32_t n_spans,
+                          uint64_t *out_n, lb2_inflate_stats *stats, uint32_t *n_table, uint32_t *n_refused);
 void lb2_inflate_destroy(lb2_inflate *d);
 
 /* ---- zip reader: every member of a zip decoded and checked on the GPU in one batch ------------------ */
@@ -419,6 +446,16 @@ int lb2_unzip_read(lb2_unzip *u, void *h_out, uint64_t cap);
  * lb2_zip_submit_device takes as a source.  Valid until the next lb2_unzip_run or lb2_unzip_destroy.  LB2_E_STATE
  * without a successful run. */
 int lb2_unzip_device_output(lb2_unzip *u, const void **d_out, uint64_t *n);
+/* lb2_unzip_run with seek tables (seek_table.py): member i's entries are spans[span_first[i] .. span_first[i + 1])
+ * (none: no table; span_first has n_members + 1 entries).  A DEFLATE member larger than one span whose entries add up
+ * to its body and size is decoded from its table as in lb2_inflate_run_table, in one launch with every other table
+ * member's spans; members without a table, with a table that is refused before or after the decode, and one-span
+ * members (decoded whole by one thread, no search to save) take the path they take in lb2_unzip_run, in the same
+ * batch and into the same output.  Results, statuses and CRC-32s are lb2_unzip_run's; *n_table / *n_refused (may be
+ * NULL) count the members decoded from a table and the tables refused. */
+int lb2_unzip_run_table(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_member *members, uint32_t n_members,
+                        const uint32_t *span_first, const lb2_inflate_span *spans, uint64_t *out_n,
+                        lb2_unzip_result *results, lb2_unzip_stats *stats, uint32_t *n_table, uint32_t *n_refused);
 void lb2_unzip_destroy(lb2_unzip *u);
 
 /* ---- tar index: the bytes tarfile reads to list the members of a tar stream in device memory ---------------- */

@@ -30,6 +30,7 @@ EXPORTS = [
     "lb2_unzip_create", "lb2_unzip_run", "lb2_unzip_read", "lb2_unzip_destroy",
     "lb2_zip_submit_device", "lb2_unzip_device_output",
     "lb2_inflate_device_output", "lb2_memcpy_d2d", "lb2_gzip_submit_device", "lb2_tar_index",
+    "lb2_gzip_chunk_sizes", "lb2_inflate_run_table", "lb2_zip_chunk_sizes", "lb2_unzip_run_table",
 ]
 TAR_STOP_ZERO, TAR_STOP_BAD_HEADER, TAR_STOP_END, TAR_STOP_UNSUPPORTED = 1, 2, 3, 4
 ZIP_CONTINUES, ZIP_MORE = 1, 2
@@ -114,6 +115,10 @@ class InflateStats(C.Structure):
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class InflateSpan(C.Structure):
+    _fields_ = [("in_len", C.c_uint64), ("out_len", C.c_uint64)]
 
 
 class UnzipMember(C.Structure):
@@ -272,6 +277,18 @@ def load():
     lib.lb2_tar_index.argtypes = [vp, vp, C.c_uint64, C.POINTER(TarRange), C.c_uint32, C.POINTER(C.c_uint32), vp,
                                   C.c_uint64, u64p, C.POINTER(TarIndexStats)]
     lib.lb2_tar_index.restype = C.c_int
+    u32p = C.POINTER(C.c_uint32)
+    lib.lb2_gzip_chunk_sizes.argtypes = [vp, u32p, C.c_uint32, u32p]
+    lib.lb2_gzip_chunk_sizes.restype = C.c_int
+    lib.lb2_inflate_run_table.argtypes = [vp, vp, C.c_uint64, C.POINTER(InflateSpan), C.c_uint32, u64p,
+                                          C.POINTER(InflateStats), u32p, u32p]
+    lib.lb2_inflate_run_table.restype = C.c_int
+    lib.lb2_zip_chunk_sizes.argtypes = [vp, u32p, C.c_uint32, u32p]
+    lib.lb2_zip_chunk_sizes.restype = C.c_int
+    lib.lb2_unzip_run_table.argtypes = [vp, vp, C.c_uint64, C.POINTER(UnzipMember), C.c_uint32, u32p,
+                                        C.POINTER(InflateSpan), u64p, C.POINTER(UnzipResult), C.POINTER(UnzipStats),
+                                        u32p, u32p]
+    lib.lb2_unzip_run_table.restype = C.c_int
     _lib = lib
     return lib
 

@@ -499,6 +499,7 @@ struct GzSlot {
   cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // upload | deflate | best | crc | compact |
   cudaEvent_t done = nullptr;
   uint32_t n_segs = 0;
+  uint32_t n_chunks = 0;
 };
 
 struct GzWriter {
@@ -514,6 +515,8 @@ struct GzWriter {
   int head = 0, count = 0;     // pieces in flight, collected in submission order
   bool finished = false;
   lb2_gzip_stats st{};
+  int sizes_slot = -1;         // the slot of the piece collected last while its chunk sizes are still in d_meta
+  uint32_t sizes_n = 0;        // its chunk count
 };
 struct lb2_gzip : GzWriter {};
 struct lb2_zip : GzWriter {};
@@ -612,7 +615,9 @@ static int gz_submit(GzWriter *g, const void *h_in, const lb2_zip_source *d_src,
                      bool last_ends) {
   lb2_ctx *ctx = g->ctx;
   CK(cudaSetDevice(ctx->device));
-  GzSlot &s = g->slot[(g->head + g->count) & 1];
+  const int slot = (g->head + g->count) & 1;
+  GzSlot &s = g->slot[slot];
+  if (g->sizes_slot == slot) g->sizes_slot = -1;
   uint64_t n_chunks = 0;
   for (uint32_t i = 0; i < n_segs; i++) n_chunks += seg_len[i] ? (seg_len[i] + GZ_CHUNK - 1) / GZ_CHUNK : 1;
   if (n_chunks > UINT32_MAX / 2) { ctx->err = "piece too large"; return LB2_E_ARG; }
@@ -701,6 +706,7 @@ static int gz_submit(GzWriter *g, const void *h_in, const lb2_zip_source *d_src,
   g->st.n_chunks += n_data;
   g->st.in_bytes += n;
   s.n_segs = n_segs;
+  s.n_chunks = c;
   g->count++;
   return LB2_OK;
 }
@@ -734,6 +740,8 @@ static int gz_collect(GzWriter *g, void *h_out, uint64_t out_cap, uint64_t *out_
     if (segs) std::copy(s.h_seg, s.h_seg + s.n_segs, segs);
   }
   *out_n = total;
+  g->sizes_slot = g->head;
+  g->sizes_n = s.n_segs ? s.n_chunks : 0;
   s.n_segs = 0;
   g->head ^= 1;
   g->count--;
@@ -805,6 +813,20 @@ int lb2_gzip_collect(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n
   if (!out_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
   if (!g->count) { ctx->err = "no piece in flight"; return LB2_E_STATE; }
   return gz_collect(g, h_out, out_cap, out_n, nullptr);
+}
+
+int lb2_gzip_chunk_sizes(lb2_gzip *g, uint32_t *sizes, uint32_t cap, uint32_t *n_chunks) {
+  if (!g) return LB2_E_ARG;
+  lb2_ctx *ctx = g->ctx;
+  if (!n_chunks) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  *n_chunks = 0;
+  if (g->sizes_slot < 0) { ctx->err = "lb2_gzip_chunk_sizes: no piece collected since the last submit into its slot"; return LB2_E_STATE; }
+  *n_chunks = g->sizes_n;
+  if (cap < g->sizes_n) { ctx->err = "lb2_gzip_chunk_sizes: buffer smaller than the piece's chunk count"; return LB2_E_CAPACITY; }
+  if (!sizes && g->sizes_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  if (g->sizes_n) CK(cudaMemcpy(sizes, g->slot[g->sizes_slot].d_meta, g->sizes_n * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  return LB2_OK;
 }
 
 int lb2_gzip_finish(lb2_gzip *g, void *h_out, uint64_t out_cap, uint64_t *out_n, uint32_t *crc32, uint64_t *isize,
@@ -896,6 +918,10 @@ int lb2_zip_submit_device(lb2_zip *z, const lb2_zip_source *src, uint32_t n_segs
   }
   return gz_submit(z, nullptr, src, n_segs, off.data(), true, n, off.data(), len.data(), n_segs, flags & LB2_ZIP_CONTINUES,
                    !(flags & LB2_ZIP_MORE));
+}
+
+int lb2_zip_chunk_sizes(lb2_zip *z, uint32_t *sizes, uint32_t cap, uint32_t *n_chunks) {
+  return lb2_gzip_chunk_sizes(reinterpret_cast<lb2_gzip *>(static_cast<GzWriter *>(z)), sizes, cap, n_chunks);
 }
 
 int lb2_zip_collect(lb2_zip *z, void *h_out, uint64_t out_cap, uint64_t *out_n, lb2_zip_segment *segs, lb2_gzip_stats *stats) {
@@ -997,32 +1023,63 @@ void lb2_inflate_destroy(lb2_inflate *d) {
   delete d;
 }
 
-int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_n, lb2_inflate_stats *stats) {
-  if (!d) return LB2_E_ARG;
+}  // extern "C"
+
+// The table path: one exact-stop span per entry, decoded into the arena with its result; true when Table::accept takes
+// the results (d_jobs then holds the laid-out spans).  A table that does not fit on the device is refused like one
+// that does not chain.
+static int ifl_table(lb2_inflate *d, uint64_t n, const lb2_inflate_span *spans, uint32_t n_spans, ifl::Table &t,
+                     lb2_inflate_stats &st, bool &accepted) {
   lb2_ctx *ctx = d->ctx;
-  if ((!h_in && n) || !out_n) { ctx->err = "NULL argument"; return LB2_E_ARG; }
-  CK(cudaSetDevice(ctx->device));
-  d->have = false;
-  *out_n = 0;
-  lb2_inflate_stats st{};
+  cudaStream_t s = d->stream;
+  accepted = false;
+  static_assert(sizeof(lb2_inflate_span) == sizeof(ifl::TableEntry), "seek-table entries");
+  if (!t.init(reinterpret_cast<const ifl::TableEntry *>(spans), n_spans, n)) return LB2_OK;
+  const uint64_t total = t.out_total;
+  const uint64_t cap_arena = d->cap_arena;
+  // a refused table leaves no trace: not its error message, nor output buffers grown to what it claimed (up to
+  // MAX_RATIO x the input), which the search then allocates for the stream's real size
+  auto refuse = [&]() {
+    ctx->err.clear();
+    if (d->cap_arena > cap_arena) {
+      cudaFree(d->d_arena); cudaFree(d->d_out); cudaFree(d->d_chunk_crc);
+      d->d_arena = nullptr; d->d_out = nullptr; d->d_chunk_crc = nullptr;
+      d->cap_arena = d->cap_out = d->cap_chunks = 0;
+    }
+    return LB2_OK;
+  };
+  if (ifl_grow(ctx, &d->d_jobs, d->cap_jobs, n_spans) || ifl_grow(ctx, &d->d_res, d->cap_res, n_spans) ||
+      ifl_grow(ctx, &d->d_arena, d->cap_arena, total) || ifl_grow(ctx, &d->d_out, d->cap_out, total) ||
+      ifl_grow(ctx, &d->d_chunk_crc, d->cap_chunks, (total + GZ_CHUNK - 1) / GZ_CHUNK + 1))
+    return refuse();
+  std::vector<ifl::SpanResult> res(n_spans);
+  CK(cudaMemcpyAsync(d->d_jobs, t.job.data(), n_spans * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
+  CK(cudaEventRecord(d->ev[0], s));
+  launch_inflate_table_decode(d->d_in, d->d_jobs, n_spans, d->d_arena, d->d_res, s);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(d->ev[1], s));
+  CK(cudaMemcpyAsync(res.data(), d->d_res, n_spans * sizeof(ifl::SpanResult), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  st.decode_ms += ifl_elapsed(d);
+  accepted = t.accept(res.data());
+  return accepted ? LB2_OK : refuse();
+}
+
+// The search path: candidates, count rounds and chain, then the decode of the confirmed spans into the arena.
+// *total is the stream's output; d_jobs holds the laid-out spans.
+static int ifl_search(lb2_inflate *d, uint64_t n, lb2_inflate_stats &st, std::vector<ifl::SpanJob> &used, uint64_t *total) {
+  lb2_ctx *ctx = d->ctx;
+  cudaStream_t s = d->stream;
   uint64_t span;
   if (!ifl_span(ctx, span)) return LB2_E_ARG;
   const uint32_t n_spans = n > span ? (uint32_t)((n + span - 1) / span) : 1;
-  cudaStream_t s = d->stream;
   int rc;
-  if ((rc = ifl_grow(ctx, &d->d_in, d->cap_in, n)) || (rc = ifl_grow(ctx, &d->d_cand, d->cap_cand, n_spans)) ||
-      (rc = ifl_grow(ctx, &d->d_jobs, d->cap_jobs, n_spans)) || (rc = ifl_grow(ctx, &d->d_res, d->cap_res, n_spans)) ||
-      (rc = ifl_grow(ctx, &d->d_find, d->cap_find, n_spans)))
+  if ((rc = ifl_grow(ctx, &d->d_cand, d->cap_cand, n_spans)) || (rc = ifl_grow(ctx, &d->d_jobs, d->cap_jobs, n_spans)) ||
+      (rc = ifl_grow(ctx, &d->d_res, d->cap_res, n_spans)) || (rc = ifl_grow(ctx, &d->d_find, d->cap_find, n_spans)))
     return rc;
   std::vector<ifl::FindJob> find;  // the one stream's nominal spans k >= 1
   for (uint32_t k = 1; k < n_spans; k++) find.push_back(ifl::FindJob{0, n, k, 0});
-  if (!find.empty()) CK(cudaMemcpyAsync(d->d_find, find.data(), find.size() * sizeof(ifl::FindJob), cudaMemcpyHostToDevice, d->stream));
-  // upload
-  CK(cudaEventRecord(d->ev[0], s));
-  if (n) CK(cudaMemcpyAsync(d->d_in, h_in, n, cudaMemcpyHostToDevice, s));
-  CK(cudaEventRecord(d->ev[1], s));
-  CK(cudaEventSynchronize(d->ev[1]));
-  st.h2d_ms = ifl_elapsed(d);
+  if (!find.empty()) CK(cudaMemcpyAsync(d->d_find, find.data(), find.size() * sizeof(ifl::FindJob), cudaMemcpyHostToDevice, s));
   // candidates
   std::vector<uint64_t> cand(n_spans, ifl::KEY_NONE);
   CK(cudaEventRecord(d->ev[0], s));
@@ -1058,19 +1115,15 @@ int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_
   st.n_absorbed = c.n_absorbed;
   if (c.error) {
     ctx->err = "lb2_inflate_run: invalid DEFLATE stream (span status " + std::to_string(c.error) + ")";
-    if (stats) *stats = st;
     return LB2_E_DATA;
   }
-  const uint64_t total = c.layout();
+  *total = c.layout();
   const uint32_t n_used = (uint32_t)c.job.size();
-  st.n_spans = n_used;
   st.in_bytes = c.in_bytes();
-  st.out_bytes = total;
   // 2 bytes per output byte for the u16 arena, 1 for the final bytes
-  if ((rc = ifl_grow(ctx, &d->d_arena, d->cap_arena, total)) || (rc = ifl_grow(ctx, &d->d_out, d->cap_out, total)) ||
-      (rc = ifl_grow(ctx, &d->d_chunk_crc, d->cap_chunks, (total + GZ_CHUNK - 1) / GZ_CHUNK + 1)))
+  if ((rc = ifl_grow(ctx, &d->d_arena, d->cap_arena, *total)) || (rc = ifl_grow(ctx, &d->d_out, d->cap_out, *total)) ||
+      (rc = ifl_grow(ctx, &d->d_chunk_crc, d->cap_chunks, (*total + GZ_CHUNK - 1) / GZ_CHUNK + 1)))
     return rc;
-  // decode, resolve, CRC-32
   CK(cudaMemcpyAsync(d->d_jobs, c.job.data(), n_used * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
   CK(cudaMemsetAsync(d->d_err, 0, sizeof(int32_t), s));
   CK(cudaEventRecord(d->ev[0], s));
@@ -1078,7 +1131,57 @@ int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_
   CK(cudaGetLastError());
   CK(cudaEventRecord(d->ev[1], s));
   CK(cudaEventSynchronize(d->ev[1]));
-  st.decode_ms = ifl_elapsed(d);
+  st.decode_ms += ifl_elapsed(d);
+  used.swap(c.job);
+  return LB2_OK;
+}
+
+// lb2_inflate_run (no table) and lb2_inflate_run_table: upload, the table path if there is a table, the search path
+// if there is none or it was refused, then resolve and CRC-32.
+static int ifl_run(lb2_inflate *d, const void *h_in, uint64_t n, const lb2_inflate_span *spans, uint32_t n_table_spans,
+                   uint64_t *out_n, lb2_inflate_stats *stats, uint32_t *n_table, uint32_t *n_refused) {
+  if (!d) return LB2_E_ARG;
+  lb2_ctx *ctx = d->ctx;
+  if ((!h_in && n) || !out_n || (!spans && n_table_spans)) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  d->have = false;
+  *out_n = 0;
+  if (n_table) *n_table = 0;
+  if (n_refused) *n_refused = 0;
+  lb2_inflate_stats st{};
+  uint64_t span;
+  if (!ifl_span(ctx, span)) return LB2_E_ARG;
+  cudaStream_t s = d->stream;
+  int rc;
+  if ((rc = ifl_grow(ctx, &d->d_in, d->cap_in, n))) return rc;
+  // upload
+  CK(cudaEventRecord(d->ev[0], s));
+  if (n) CK(cudaMemcpyAsync(d->d_in, h_in, n, cudaMemcpyHostToDevice, s));
+  CK(cudaEventRecord(d->ev[1], s));
+  CK(cudaEventSynchronize(d->ev[1]));
+  st.h2d_ms = ifl_elapsed(d);
+  bool accepted = false;
+  ifl::Table t;
+  if (n_table_spans) {
+    if ((rc = ifl_table(d, n, spans, n_table_spans, t, st, accepted))) return rc;
+    if (n_table) *n_table = accepted;
+    if (n_refused) *n_refused = !accepted;
+  }
+  std::vector<ifl::SpanJob> used;
+  uint64_t total = 0;
+  if (accepted) {
+    used.swap(t.job);
+    total = t.out_total;
+    st.in_bytes = t.in_total;
+    CK(cudaMemsetAsync(d->d_err, 0, sizeof(int32_t), s));
+  } else if ((rc = ifl_search(d, n, st, used, &total))) {
+    if (stats) *stats = st;
+    return rc;
+  }
+  const uint32_t n_used = (uint32_t)used.size();
+  st.n_spans = n_used;
+  st.out_bytes = total;
+  // resolve, CRC-32
   CK(cudaEventRecord(d->ev[0], s));
   const uint32_t span_range[2] = {0, n_used};
   CK(cudaMemcpyAsync(d->d_first, span_range, sizeof span_range, cudaMemcpyHostToDevice, s));
@@ -1105,6 +1208,17 @@ int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_
   d->have = true;
   *out_n = total;
   return LB2_OK;
+}
+
+extern "C" {
+
+int lb2_inflate_run(lb2_inflate *d, const void *h_in, uint64_t n, uint64_t *out_n, lb2_inflate_stats *stats) {
+  return ifl_run(d, h_in, n, nullptr, 0, out_n, stats, nullptr, nullptr);
+}
+
+int lb2_inflate_run_table(lb2_inflate *d, const void *h_in, uint64_t n, const lb2_inflate_span *spans, uint32_t n_spans,
+                          uint64_t *out_n, lb2_inflate_stats *stats, uint32_t *n_table, uint32_t *n_refused) {
+  return ifl_run(d, h_in, n, spans, n_spans, out_n, stats, n_table, n_refused);
 }
 
 int lb2_inflate_device_output(lb2_inflate *d, const void **d_out, uint64_t *n) {
@@ -1197,11 +1311,22 @@ void lb2_unzip_destroy(lb2_unzip *u) {
   delete u;
 }
 
-int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_member *members, uint32_t n_members,
-                  uint64_t *out_n, lb2_unzip_result *results, lb2_unzip_stats *stats) {
+}  // extern "C"
+
+// lb2_unzip_run (no tables) and lb2_unzip_run_table: members with an accepted seek table are decoded from it and
+// resolved with the search path's spans; every other member (a refused table's included) takes the path it takes
+// without one.
+static int uz_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_member *members, uint32_t n_members,
+                  const uint32_t *span_first, const lb2_inflate_span *spans, uint64_t *out_n, lb2_unzip_result *results,
+                  lb2_unzip_stats *stats, uint32_t *n_table, uint32_t *n_refused) {
   if (!u) return LB2_E_ARG;
   lb2_ctx *ctx = u->ctx;
-  if ((!h_in && n) || !out_n || (n_members && (!members || !results))) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  if ((!h_in && n) || !out_n || (n_members && (!members || !results)) || (span_first && !spans && span_first[n_members])) {
+    ctx->err = "NULL argument";
+    return LB2_E_ARG;
+  }
+  if (n_table) *n_table = 0;
+  if (n_refused) *n_refused = 0;
   u->have = false;
   *out_n = 0;
   // everything the archive says is checked before any launch
@@ -1224,7 +1349,27 @@ int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_me
   lb2_unzip_stats st{};
   st.n_members = n_members;
   st.in_bytes = n;
-  ifl::Batch b;
+  // seek tables, checked on the host: a DEFLATE member that would take the search pipeline (more than one span) and
+  // whose entries add up to its body and recorded size.  A one-span member is decoded whole by one thread anyway.
+  std::vector<uint8_t> tabled(n_members, 0);
+  std::vector<ifl::Table> tables;
+  std::vector<uint32_t> table_member;
+  uint32_t refused = 0;
+  for (uint32_t i = 0; span_first && i < n_members; i++) {
+    const uint32_t k = span_first[i + 1] - span_first[i];
+    const ifl::Member &x = m[i];
+    if (!k || (x.method == 8 && x.in_len <= span)) continue;
+    ifl::Table t;
+    if (span_first[i + 1] < span_first[i] || x.method != 8 ||
+        !t.init(reinterpret_cast<const ifl::TableEntry *>(spans + span_first[i]), k, x.in_len, x.in_off, x.out_off, i) ||
+        t.in_total != x.in_len || t.out_total != x.out_len) {
+      refused++;
+      continue;
+    }
+    tables.push_back(std::move(t));
+    table_member.push_back(i);
+  }
+  ifl::Batch b;  // sized here for every member; set up again below without those a table decodes
   b.init(m.data(), n_members, span);
   st.n_stored = (uint32_t)b.stored.size();
   st.n_small = (uint32_t)b.small.size();
@@ -1254,11 +1399,48 @@ int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_me
     CK(cudaMemcpyAsync(u->d_members, m.data(), n_members * sizeof(ifl::Member), cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(u->d_status, b.status.data(), n_members * sizeof(int32_t), cudaMemcpyHostToDevice, s));
   }
+  CK(cudaStreamSynchronize(s));
+  st.h2d_ms = uz_elapsed(u);
+  // the seek-table members: one exact-stop span per entry into the arena, then Table::accept per member
+  std::vector<ifl::SpanJob> table_jobs;
+  std::vector<uint32_t> table_first{0};
+  if (!tables.empty()) {
+    std::vector<ifl::SpanJob> all;
+    for (const ifl::Table &t : tables) all.insert(all.end(), t.job.begin(), t.job.end());
+    if ((rc = ifl_grow(ctx, &u->d_arena, u->cap_arena, total, what)) || (rc = ifl_grow(ctx, &u->d_jobs, u->cap_jobs, all.size(), what)) ||
+        (rc = ifl_grow(ctx, &u->d_res, u->cap_res, all.size(), what)))
+      return rc;
+    std::vector<ifl::SpanResult> res(all.size());
+    CK(cudaMemcpyAsync(u->d_jobs, all.data(), all.size() * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(u->ev[0], s));
+    launch_inflate_table_decode(u->d_in, u->d_jobs, (uint32_t)all.size(), u->d_arena, u->d_res, s);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(u->ev[1], s));
+    CK(cudaMemcpyAsync(res.data(), u->d_res, res.size() * sizeof(ifl::SpanResult), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    st.decode_ms += uz_elapsed(u);
+    size_t at = 0;
+    for (size_t i = 0; i < tables.size(); i++) {
+      if (tables[i].accept(res.data() + at)) {
+        tabled[table_member[i]] = 1;
+        table_jobs.insert(table_jobs.end(), tables[i].job.begin(), tables[i].job.end());
+        table_first.push_back((uint32_t)table_jobs.size());
+      } else {
+        refused++;
+      }
+      at += tables[i].job.size();
+    }
+  }
+  if (n_table) *n_table = (uint32_t)table_first.size() - 1;
+  if (n_refused) *n_refused = refused;
+  if (table_first.size() > 1) {  // the accepted members leave every other path (the buffers above are large enough)
+    b.init(m.data(), n_members, span, tabled.data());
+    st.n_small = (uint32_t)b.small.size();
+    st.n_large = (uint32_t)b.large.size();
+  }
   if (!b.stored.empty()) CK(cudaMemcpyAsync(u->d_idx, b.stored.data(), b.stored.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
   if (!b.small.empty()) CK(cudaMemcpyAsync(u->d_small, b.small.data(), b.small.size() * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
   if (!b.find.empty()) CK(cudaMemcpyAsync(u->d_find, b.find.data(), b.find.size() * sizeof(ifl::FindJob), cudaMemcpyHostToDevice, s));
-  CK(cudaStreamSynchronize(s));
-  st.h2d_ms = uz_elapsed(u);
   // STORED members, then the one-span members
   CK(cudaEventRecord(u->ev[0], s));
   launch_unzip_copy(u->d_in, u->d_members, u->d_idx, (uint32_t)b.stored.size(), u->d_out, s);
@@ -1273,6 +1455,8 @@ int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_me
   CK(cudaEventSynchronize(u->ev[1]));
   st.small_ms = uz_elapsed(u);
   // larger members: candidates, then count rounds with one chain per member
+  std::vector<ifl::SpanJob> jobs;
+  std::vector<uint32_t> first{0};
   if (!b.large.empty()) {
     std::vector<uint64_t> cand(b.find.size());
     CK(cudaEventRecord(u->ev[0], s));
@@ -1283,7 +1467,6 @@ int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_me
     CK(cudaStreamSynchronize(s));
     st.find_ms = uz_elapsed(u);
     b.start_chains(cand.data(), span);
-    std::vector<ifl::SpanJob> jobs;
     std::vector<ifl::SpanResult> res;
     std::vector<std::pair<uint32_t, uint32_t>> ref;
     while (b.pending(jobs, ref)) {
@@ -1303,30 +1486,34 @@ int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_me
     st.n_rounds = b.n_rounds;
     st.n_rejected = b.n_rejected();
     st.n_absorbed = b.n_absorbed();
-    // decode the members whose chains ended at their recorded sizes into the u16 arena at their output offsets
-    std::vector<uint32_t> first;
+    // the members whose chains ended at their recorded sizes
     b.layout(jobs, first);
-    st.n_spans = (uint32_t)jobs.size();
-    const uint32_t n_dec = (uint32_t)first.size() - 1;
-    if (n_dec) {
-      if ((rc = ifl_grow(ctx, &u->d_arena, u->cap_arena, total, what)) || (rc = ifl_grow(ctx, &u->d_jobs, u->cap_jobs, jobs.size(), what)) ||
-          (rc = ifl_grow(ctx, &u->d_first, u->cap_first, first.size(), what)))
-        return rc;
-      CK(cudaMemcpyAsync(u->d_jobs, jobs.data(), jobs.size() * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
-      CK(cudaMemcpyAsync(u->d_first, first.data(), first.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-      CK(cudaEventRecord(u->ev[0], s));
-      launch_inflate_decode(u->d_in, u->d_jobs, (uint32_t)jobs.size(), u->d_arena, u->d_status, s);
-      CK(cudaGetLastError());
-      CK(cudaEventRecord(u->ev[1], s));
-      CK(cudaEventSynchronize(u->ev[1]));
-      st.decode_ms = uz_elapsed(u);
-      CK(cudaEventRecord(u->ev[0], s));
-      launch_inflate_resolve(u->d_arena, u->d_out, u->d_jobs, (uint32_t)jobs.size(), u->d_first, n_dec, u->d_status, s);
-      CK(cudaGetLastError());
-      CK(cudaEventRecord(u->ev[1], s));
-      CK(cudaEventSynchronize(u->ev[1]));
-      st.resolve_ms = uz_elapsed(u);
-    }
+  }
+  // decode the search path's spans into the u16 arena at their output offsets, then resolve them with the accepted
+  // seek-table members' spans (decoded above)
+  const uint32_t n_search = (uint32_t)jobs.size();
+  for (size_t i = 1; i < table_first.size(); i++) first.push_back(n_search + table_first[i]);
+  jobs.insert(jobs.end(), table_jobs.begin(), table_jobs.end());
+  st.n_spans = (uint32_t)jobs.size();
+  const uint32_t n_dec = (uint32_t)first.size() - 1;
+  if (n_dec) {
+    if ((rc = ifl_grow(ctx, &u->d_arena, u->cap_arena, total, what)) || (rc = ifl_grow(ctx, &u->d_jobs, u->cap_jobs, jobs.size(), what)) ||
+        (rc = ifl_grow(ctx, &u->d_first, u->cap_first, first.size(), what)))
+      return rc;
+    CK(cudaMemcpyAsync(u->d_jobs, jobs.data(), jobs.size() * sizeof(ifl::SpanJob), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(u->d_first, first.data(), first.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    CK(cudaEventRecord(u->ev[0], s));
+    launch_inflate_decode(u->d_in, u->d_jobs, n_search, u->d_arena, u->d_status, s);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(u->ev[1], s));
+    CK(cudaEventSynchronize(u->ev[1]));
+    st.decode_ms += uz_elapsed(u);
+    CK(cudaEventRecord(u->ev[0], s));
+    launch_inflate_resolve(u->d_arena, u->d_out, u->d_jobs, (uint32_t)jobs.size(), u->d_first, n_dec, u->d_status, s);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(u->ev[1], s));
+    CK(cudaEventSynchronize(u->ev[1]));
+    st.resolve_ms = uz_elapsed(u);
   }
   // CRC-32 of every member: the writer's chunk table over the output, one segment per member
   std::vector<GzSegResult> seg(n_members);
@@ -1377,6 +1564,20 @@ int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_me
   u->have = true;
   *out_n = total;
   return LB2_OK;
+}
+
+extern "C" {
+
+int lb2_unzip_run(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_member *members, uint32_t n_members,
+                  uint64_t *out_n, lb2_unzip_result *results, lb2_unzip_stats *stats) {
+  return uz_run(u, h_in, n, members, n_members, nullptr, nullptr, out_n, results, stats, nullptr, nullptr);
+}
+
+int lb2_unzip_run_table(lb2_unzip *u, const void *h_in, uint64_t n, const lb2_unzip_member *members, uint32_t n_members,
+                        const uint32_t *span_first, const lb2_inflate_span *spans, uint64_t *out_n,
+                        lb2_unzip_result *results, lb2_unzip_stats *stats, uint32_t *n_table, uint32_t *n_refused) {
+  if (u && !span_first) { u->ctx->err = "NULL argument"; return LB2_E_ARG; }
+  return uz_run(u, h_in, n, members, n_members, span_first, spans, out_n, results, stats, n_table, n_refused);
 }
 
 int lb2_unzip_device_output(lb2_unzip *u, const void **d_out, uint64_t *n) {

@@ -5,6 +5,8 @@
 //            lowest passing one is the span's candidate;
 //   count    one thread per span, tables in shared memory: decode without writing, record the end key and length;
 //   decode   one thread per confirmed span: the same walk, writing the u16 arena;
+//   table    one thread per seek-table span (exact stop): the decode walk, also writing each span's result, which the
+//            host checks before it trusts the table;
 //   window   one CTA per stream walks its spans in order and makes the last 32 KB of each final (the next span's window);
 //   resolve  one CTA per span makes the rest final, reading marker values from the windows;
 //   small    (zip reader) one thread per stream of at most one span: the byte-output walk, straight into the output;
@@ -69,6 +71,19 @@ __global__ void __launch_bounds__(SPAN_THREADS) lb2_inflate_decode_kernel(const 
   SpanResult r;
   decode_span<true>(in + j.in_off, j.in_n, j, st, arena + j.out_off, r);
   if (r.status != ifl::ST_OK) atomicExch(err + j.member, r.status);
+}
+
+__global__ void __launch_bounds__(SPAN_THREADS) lb2_inflate_table_decode_kernel(const uint8_t *in, const SpanJob *jobs,
+                                                                                 uint32_t n_jobs, uint16_t *arena,
+                                                                                 SpanResult *res) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  DecodeState &st = reinterpret_cast<DecodeState *>(smem)[threadIdx.x];
+  const uint32_t i = blockIdx.x * SPAN_THREADS + threadIdx.x;
+  if (i >= n_jobs) return;
+  const SpanJob j = jobs[i];
+  SpanResult r;
+  decode_span<true>(in + j.in_off, j.in_n, j, st, arena + j.out_off, r);
+  res[i] = r;
 }
 
 constexpr int32_t ERR_WINDOW = -100;  // a marker points before the stream start
@@ -143,6 +158,14 @@ void launch_inflate_decode(const uint8_t *in, const SpanJob *jobs, uint32_t n_jo
   const uint32_t smem = SPAN_THREADS * sizeof(DecodeState);
   cudaFuncSetAttribute(lb2_inflate_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   lb2_inflate_decode_kernel<<<(n_jobs + SPAN_THREADS - 1) / SPAN_THREADS, SPAN_THREADS, smem, s>>>(in, jobs, n_jobs, arena, err);
+}
+void launch_inflate_table_decode(const uint8_t *in, const SpanJob *jobs, uint32_t n_jobs, uint16_t *arena, SpanResult *res,
+                                 cudaStream_t s) {
+  if (!n_jobs) return;
+  const uint32_t smem = SPAN_THREADS * sizeof(DecodeState);
+  cudaFuncSetAttribute(lb2_inflate_table_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  lb2_inflate_table_decode_kernel<<<(n_jobs + SPAN_THREADS - 1) / SPAN_THREADS, SPAN_THREADS, smem, s>>>(in, jobs, n_jobs,
+                                                                                                         arena, res);
 }
 void launch_inflate_resolve(const uint16_t *arena, uint8_t *out, const SpanJob *jobs, uint32_t n_jobs, const uint32_t *first,
                             uint32_t n_streams, int32_t *err, cudaStream_t s) {

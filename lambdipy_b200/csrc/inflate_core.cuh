@@ -12,6 +12,12 @@
 // Keys.  A candidate's key orders block starts: bit << 2 for a block whose header is read at `bit` (dynamic blocks,
 // and span 0's first block of any type); (bit << 2) | 2 | BFINAL for a stored block whose LEN field starts at `bit`
 // (the header bits and padding in front of it may sit at several offsets, which all decode the same).
+//
+// Seek table.  A stream whose writer recorded where its blocks start (the GPU writers end every 64 KB chunk
+// byte-aligned with an empty stored block and can keep each run of chunks' compressed and decoded lengths, see
+// seek_table.py) needs no search: Table turns the entries into one exact-stop span each, decoded once straight into
+// the arena, and accepts the results only if they chain as Chain::walk requires.  A refused table costs one decode
+// pass; the caller then runs the search above on the same stream.
 #pragma once
 #include <cstdint>
 #include <utility>
@@ -42,7 +48,8 @@ enum : int32_t {
   ST_BAD_STORED = -4,   // LEN != ~NLEN
   ST_EOF = -5,          // ran past the end of the input
   ST_GIVE_UP = -6,      // an unconfirmed span ran the give-up distance past its end
-  ST_OVERFLOW = -7      // decode pass: more output than the count pass measured
+  ST_OVERFLOW = -7,     // decode pass: more output than the count pass measured
+  ST_PAST_STOP = -8     // exact stop: a block header beyond stop_bit
 };
 
 // ---- tables -------------------------------------------------------------------------------------------------------
@@ -304,7 +311,7 @@ struct SpanJob {
   uint64_t out_off;    // decode pass: where the span's output starts in the arena
   uint64_t out_len;    // decode pass: the counted length
   uint32_t first;      // span 0: no window in front of it
-  uint32_t pad;
+  uint32_t exact;      // stop at the block header (of any type) read exactly at stop_bit; one beyond it is an error
   // where the span's stream is: the kernels decode in[in_off .. in_off + in_n); out_base is the stream's first output
   // byte in the arena (a window marker must not point before it); member indexes the per-stream status
   uint64_t in_off, in_n, out_base;
@@ -358,7 +365,10 @@ IFL_HD void decode_span(const uint8_t *in, uint64_t n, const SpanJob &job, Decod
       const uint64_t hb = b.pos();
       if (hb + 3 > n * 8) { status = ST_EOF; break; }
       const uint32_t h = b.peek(3);
-      if (!first_block) {
+      if (!first_block && job.exact) {
+        if (hb == job.stop_bit) { end_key = key_header(hb); break; }
+        if (hb > job.stop_bit) { status = ST_PAST_STOP; break; }
+      } else if (!first_block) {
         if ((h >> 1) == 2 && hb >= job.stop_bit) { end_key = key_header(hb); break; }
         if ((h >> 1) == 0) {
           const uint64_t lb = (hb + 3 + 7) & ~7ull;
@@ -493,7 +503,7 @@ struct Chain {
       j.limit_bit = i == 0 ? KEY_NONE : end + (uint64_t)giveup * span_bytes * 8;
       j.out_off = j.out_len = 0;
       j.first = i == 0;
-      j.pad = 0;
+      j.exact = 0;
       j.in_off = in_off;
       j.in_n = n;
       j.out_base = 0;
@@ -573,6 +583,57 @@ struct Chain {
   uint64_t in_bytes() const { return job.empty() ? 0 : (res.back().end_bit + 7) / 8; }
 };
 
+// ---- seek table (host) -------------------------------------------------------------------------------------------
+// Entry e covers in[in_len of the entries before it .. + e.in_len) and decodes to e.out_len bytes; every entry after
+// the first starts with a block header at its first byte.  The entries come from outside the program, so init refuses
+// any that could not describe the stream: a zero length, more than MAX_RATIO output bytes per input byte (258-byte
+// matches of 2 bits each), or more input than the n bytes there are.  A refused init allocates nothing.
+constexpr uint64_t MAX_RATIO = 1032;
+struct TableEntry {
+  uint64_t in_len, out_len;
+};
+struct Table {
+  std::vector<SpanJob> job;
+  uint64_t in_total = 0, out_total = 0;
+
+  // the stream is in[in_off .. in_off + n) of the kernels' input, its output starts at out_base of the arena
+  bool init(const TableEntry *e, uint32_t n_entries, uint64_t n, uint64_t in_off = 0, uint64_t out_base = 0,
+            uint32_t member = 0) {
+    job.clear();
+    in_total = out_total = 0;
+    if (!n_entries) return false;
+    for (uint32_t i = 0; i < n_entries; i++) {
+      if (!e[i].in_len || !e[i].out_len || e[i].in_len > n - in_total || (e[i].out_len - 1) / MAX_RATIO >= e[i].in_len ||
+          e[i].out_len > ~0ull / 4 - out_total)
+        return false;
+      in_total += e[i].in_len;
+      out_total += e[i].out_len;
+    }
+    job.resize(n_entries);
+    uint64_t in = 0, out = 0;
+    for (uint32_t i = 0; i < n_entries; i++) {
+      const uint64_t end = (in + e[i].in_len) * 8;
+      job[i] = SpanJob{key_header(in * 8), i + 1 < n_entries ? end : KEY_NONE, end, out_base + out, e[i].out_len,
+                       i == 0, 1, in_off, n, out_base, member, 0};
+      in += e[i].in_len;
+      out += e[i].out_len;
+    }
+    return true;
+  }
+  // The chain argument of Chain::walk: every span decoded exactly its length and stopped at the header the next one
+  // starts from, only the last one decoded the final block and it ended with the table's last byte.  Accepted spans
+  // are therefore the serial decode of the stream cut at the table's boundaries.
+  bool accept(const SpanResult *r) const {
+    for (size_t i = 0; i < job.size(); i++) {
+      const bool last = i + 1 == job.size();
+      if (r[i].status != ST_OK || r[i].out_len != job[i].out_len || r[i].final != (last ? 1u : 0u)) return false;
+      if (!last && r[i].end_key != job[i + 1].start_key) return false;
+      if (last && (r[i].end_bit + 7) / 8 != in_total) return false;
+    }
+    return !job.empty();
+  }
+};
+
 // ---- member table (host): many streams decoded in one batch (the zip reader) --------------------------------------
 // Each member is a raw DEFLATE (method 8) or STORED (method 0) body in[in_off .. in_off + in_len) whose output goes to
 // out[out_off .. out_off + out_len), out_len being the size the archive records.  A DEFLATE body of at most one span
@@ -600,7 +661,8 @@ struct Batch {
   std::vector<Chain> chain;               // per large member
   uint32_t n_rounds = 0;
 
-  void init(const Member *members, uint32_t n, uint64_t span) {
+  // skip (may be null): members already decoded from a seek table, left out of every path here
+  void init(const Member *members, uint32_t n, uint64_t span, const uint8_t *skip = nullptr) {
     m.assign(members, members + n);
     status.assign(n, MS_OK);
     stored.clear(); small.clear(); large.clear(); find.clear(); chain.clear();
@@ -608,6 +670,7 @@ struct Batch {
     n_rounds = 0;
     for (uint32_t i = 0; i < n; i++) {
       const Member &x = m[i];
+      if (skip && skip[i]) continue;
       if (x.method == 0) {
         if (x.in_len != x.out_len) status[i] = MS_WRONG_SIZE;
         else stored.push_back(i);

@@ -22,6 +22,11 @@ fails the build, and the line gains the member count.  No other value is accepte
 
 With LAMBDIPY_DEFLATE_LEVEL=9 (default: unset, the default encoder) the GPU tarball mirror and the bundle zip use
 the thorough encoder (an optimal parse; smaller output, longer kernels).  No other value is accepted.
+
+With LAMBDIPY_SEEK_TABLE=1 (default: unset, nothing changes) the GPU tarball mirror appends a seek table to the
+package tarball (tarball.GpuGzipFile) and the bundle zip gives its members seek tables (zipfile_gpu.zip_tree), so
+that every later read on the GPU -- the extraction of the tarball, LAMBDIPY_BUNDLE_VERIFY's read-back of the bundle --
+decodes them without searching for block starts.  No other value is accepted.
 """
 import os
 import sys
@@ -62,16 +67,25 @@ def bundle_verify():
     return True
 
 
-def zip_after_copy(copy_include_paths, zip_path, compresslevel=None, verify=False):
+def seek_table():
+    """LAMBDIPY_SEEK_TABLE, checked: False when unset, True for 1."""
+    v = os.environ.get("LAMBDIPY_SEEK_TABLE")
+    if v is None:
+        return False
+    if v != "1":
+        raise ValueError("LAMBDIPY_SEEK_TABLE=%r: expected 1 (write a seek table into the package tarball) or unset" % v)
+    return True
+
+
+def zip_after_copy(copy_include_paths, zip_path, compresslevel=None, verify=False, seek=False):
     """copy_include_paths followed by the bundle zip of its build directory, with verify its read-back check, and the
     size line."""
     def wrapped(include_paths, build_directory="./build"):
         copy_include_paths(include_paths, build_directory)
         from . import project_build, zipfile_gpu
-        if compresslevel is None:
-            zipfile_gpu.zip_tree(build_directory, zip_path)
-        else:
-            zipfile_gpu.zip_tree(build_directory, zip_path, compresslevel=compresslevel)
+        from .seek_table import seek_kw
+        level = {} if compresslevel is None else {"compresslevel": compresslevel}
+        zipfile_gpu.zip_tree(build_directory, zip_path, **level, **seek_kw(seek))
         checked = ""
         if verify:
             bad = zipfile_gpu.testzip(zip_path)
@@ -96,6 +110,7 @@ def apply():
     zip_path = bundle_zip_path()
     level = deflate_level()
     verify = bundle_verify()
+    seek = seek_table()
     import lambdipy.cli as cli
     import lambdipy.project_build as ref
     from . import project_build as mine
@@ -104,15 +119,13 @@ def apply():
     if backend == "b200":
         import lambdipy.package_build as ref_pkg
         from . import tarball
-        ref_pkg.PackageBuild.create_compressed_tarball = tarball.tarball_method(level)
+        from .seek_table import seek_kw
+        ref_pkg.PackageBuild.create_compressed_tarball = tarball.tarball_method(level, **seek_kw(seek))
     if untar == "b200":
         from . import tarball
         ref.prepare_tarfile = tarball.prepare_tarfile
     if zip_path is not None:
-        if verify:
-            cli.copy_include_paths = zip_after_copy(ref.copy_include_paths, zip_path, level, verify=True)
-        else:
-            cli.copy_include_paths = zip_after_copy(ref.copy_include_paths, zip_path, level)
+        cli.copy_include_paths = zip_after_copy(ref.copy_include_paths, zip_path, level, verify=verify, seek=seek)
     # `lambdipy build` spends seconds resolving, downloading and copying packages before it reaches the
     # strip step (cli.py:52-67): create the CUDA context behind that, not in front of the strip
     if os.environ.get("LAMBDIPY_B200_EAGER_WARMUP", "1") != "0":

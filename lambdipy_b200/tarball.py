@@ -27,7 +27,12 @@ deflated from device segments (`lb2_gzip_submit_device`).
 
     strip_tarball(src, dst)                        the .tar.gz that extracting src, the reference's
                                                    `find -name "*.so" | xargs strip` and tarfile "w:gz" would give
-    python -m lambdipy_b200.tarball strip SRC DST [--level 9]
+    python -m lambdipy_b200.tarball strip SRC DST [--level 9] [--seek-table]
+
+With seek_table=True the writers append a seek table (seek_table.py): the compressed and decoded length of every
+64 KB chunk, which the encoder computes anyway.  The readers find it from the file's tail and decode each chunk once
+from its known start (lb2_inflate_run_table) instead of searching for block starts; a table the reader does not
+accept costs one decode pass and the file is then read by the search, with the same bytes.
 """
 import ctypes as C
 import glob
@@ -44,6 +49,7 @@ import urllib.request
 import numpy as np
 
 from . import _native as N
+from . import seek_table as ST
 
 PIECE_BYTES = 64 << 20  # input per GPU submission; two pieces are in flight while the next one is filled
 
@@ -59,10 +65,14 @@ class GpuGzipFile(io.BufferedIOBase):
     any, else a new one on device LAMBDIPY_B200_DEVICE (default 0) that close() releases.
 
     compresslevel=None keeps the default encoder; 9 selects the thorough one (LB2_DEFLATE_BEST: an optimal parse,
-    never larger, slower); anything else raises ValueError."""
+    never larger, slower); anything else raises ValueError.
+
+    seek_table=True appends a seek table (seek_table.py) after the trailer when the stream has two or more entries:
+    the chunk sizes the encoder already computes, with which the GPU reader decodes the file in one pass, without
+    searching for block starts.  The bytes before it are the ones written without it."""
 
     def __init__(self, filename, mtime=None, ctx=None, piece_bytes=PIECE_BYTES, compresslevel=None, fileobj=None,
-                 host_buffers=True):
+                 host_buffers=True, seek_table=False):
         self.name = filename
         self._own_ctx = False
         self._ctx = self._g = self._out = self._file = None
@@ -92,6 +102,9 @@ class GpuGzipFile(io.BufferedIOBase):
         self._in_flight = 0
         self.offset = 0        # uncompressed bytes written
         self.stats = None
+        self._seek = bool(seek_table)
+        self._pending = []     # uncompressed bytes of each piece in flight, oldest first
+        self._chunks = []      # (compressed, uncompressed) of every collected chunk
 
     def writable(self):
         return True
@@ -118,6 +131,7 @@ class GpuGzipFile(io.BufferedIOBase):
     def _submit(self):
         ctx = self._ctx
         ctx.check(ctx.lib.lb2_gzip_submit(self._g, self._bufs[self._cur][0], self._fill))
+        self._pending.append(self._fill)
         self._in_flight += 1
         self._cur ^= 1
         self._fill = 0
@@ -137,6 +151,7 @@ class GpuGzipFile(io.BufferedIOBase):
         for i, (addr, n) in enumerate(refs):
             src[i].d_ptr, src[i].len = addr, n
         ctx.check(ctx.lib.lb2_gzip_submit_device(self._g, src, len(refs)))
+        self._pending.append(sum(n for _, n in refs))
         self._in_flight += 1
         self.offset += sum(n for _, n in refs)
         if self._in_flight == 2:  # keep one piece running while the older one is collected
@@ -148,6 +163,15 @@ class GpuGzipFile(io.BufferedIOBase):
         ctx.check(ctx.lib.lb2_gzip_collect(self._g, self._out, self._out_cap, C.byref(n)))
         self._file.write(C.string_at(self._out, n.value))
         self._in_flight -= 1
+        size = self._pending.pop(0)
+        if self._seek:
+            k = C.c_uint32()
+            sizes = (C.c_uint32 * max(-(-size // ST.CHUNK), 1))()
+            ctx.check(ctx.lib.lb2_gzip_chunk_sizes(self._g, sizes, len(sizes), C.byref(k)))
+            if k.value != -(-size // ST.CHUNK) or sum(sizes[:k.value]) != n.value:
+                raise RuntimeError("lb2_gzip_chunk_sizes: %d chunks of %d bytes for a piece of %d bytes in %d"
+                                   % (k.value, sum(sizes[:k.value]), size, n.value))
+            self._chunks += [(sizes[i], min(ST.CHUNK, size - i * ST.CHUNK)) for i in range(k.value)]
 
     def close(self):
         if self.closed:
@@ -165,6 +189,13 @@ class GpuGzipFile(io.BufferedIOBase):
                 self._file.write(C.string_at(self._out, n.value))
                 self._file.write(struct.pack("<II", crc.value, isize.value & 0xFFFFFFFF))
                 self.stats = st.as_dict()
+                if self._seek and self._chunks:
+                    c, u = self._chunks[-1]
+                    self._chunks[-1] = (c + n.value, u)   # the final block belongs to the last entry
+                    entries = ST.build(self._chunks)
+                    self.stats["seek_entries"] = len(entries) if entries else 0
+                    if entries:
+                        self._file.write(ST.gzip_member(entries, self._file.tell()))
         finally:
             self._release()
             super().close()
@@ -212,38 +243,39 @@ def gzip_header(filename, mtime=None):
     return head + (fname + b"\0" if fname else b"")
 
 
-def gzip_tarball(src_paths, tarball_path, ctx=None, compresslevel=None):
+def gzip_tarball(src_paths, tarball_path, ctx=None, compresslevel=None, seek_table=False):
     """Write `tarball_path` as a gzip-compressed tar of `src_paths`, each added recursively under its
     basename -- what `tarfile.open(tarball_path, "w:gz")` with `tar.add(p, arcname=basename(p))` writes,
-    with the same tar stream.  compresslevel: as GpuGzipFile's.  Returns tarball_path."""
+    with the same tar stream.  compresslevel, seek_table: as GpuGzipFile's.  Returns tarball_path."""
     N.deflate_flags(compresslevel)
-    with GpuGzipFile(tarball_path, ctx=ctx, compresslevel=compresslevel) as gz, tarfile.open(name=tarball_path, mode="w", fileobj=gz) as tar:
+    with GpuGzipFile(tarball_path, ctx=ctx, compresslevel=compresslevel, seek_table=seek_table) as gz, \
+            tarfile.open(name=tarball_path, mode="w", fileobj=gz) as tar:
         for path in src_paths:
             tar.add(path, arcname=os.path.basename(path))
     return tarball_path
 
 
-def create_compressed_tarball(package_build, ctx=None, compresslevel=None):
+def create_compressed_tarball(package_build, ctx=None, compresslevel=None, seek_table=False):
     """Mirror of PackageBuild.create_compressed_tarball: every top-level entry of the package's build
-    directory into ~/.lambdipy/build/<git tag>.tar.gz; returns that path.  compresslevel: as GpuGzipFile's."""
+    directory into ~/.lambdipy/build/<git tag>.tar.gz; returns that path.  compresslevel, seek_table: as
+    GpuGzipFile's."""
     N.deflate_flags(compresslevel)
     home = os.environ["HOME"]
     tarball_path = f"{home}/.lambdipy/build/{package_build.git_tag()}.tar.gz"
     srcs = glob.glob(f"{package_build.build_directory()}/*")
-    if compresslevel is None:
-        return gzip_tarball(srcs, tarball_path, ctx)
-    return gzip_tarball(srcs, tarball_path, ctx, compresslevel=compresslevel)
+    level = {} if compresslevel is None and not seek_table else {"compresslevel": compresslevel}
+    return gzip_tarball(srcs, tarball_path, ctx, **level, **ST.seek_kw(seek_table))
 
 
-def tarball_method(compresslevel):
+def tarball_method(compresslevel, seek_table=False):
     """The PackageBuild.create_compressed_tarball that patch.apply() installs: the mirror itself for the default
-    encoder, else the mirror writing at `compresslevel`."""
+    encoder without a seek table, else the mirror writing at `compresslevel`, with a seek table if asked."""
     N.deflate_flags(compresslevel)
-    if compresslevel is None:
+    if compresslevel is None and not seek_table:
         return create_compressed_tarball
 
     def create_compressed_tarball_at_level(package_build):
-        return create_compressed_tarball(package_build, compresslevel=compresslevel)
+        return create_compressed_tarball(package_build, compresslevel=compresslevel, **ST.seek_kw(seek_table))
     return create_compressed_tarball_at_level
 
 
@@ -326,11 +358,35 @@ def gunzip(path, ctx=None):
             ctx.close()
 
 
-def inflate_members(ctx, d, path, on_member):
+def _seek_spans(buf, size):
+    """(where the members end, the lb2_inflate_span table of the first member, or None): a file of exactly one data
+    member followed by a seek-table member whose entries add up to that member's body and ISIZE.  Anything else reads
+    as a file without a table (its last member, if any, is then an empty gzip member like any other)."""
+    tail = ST.gzip_tail(memoryview(buf).cast("B")) if size else None
+    if tail is None:
+        return size, None
+    end, entries = tail
+    try:
+        body = next(gzip_members(memoryview(buf).cast("B")[:end]), None)
+    except (gzip.BadGzipFile, EOFError):
+        return size, None
+    if body is None or body > end - 8 or buf[0] == 0:
+        return size, None
+    if not ST.valid(entries, end - 8 - body, struct.unpack_from("<I", buf, end - 4)[0], 0xFFFFFFFF):
+        return size, None
+    spans = (N.InflateSpan * len(entries))()
+    for i, (c, u) in enumerate(entries):
+        spans[i].in_len, spans[i].out_len = c, u
+    return end, spans
+
+
+def inflate_members(ctx, d, path, on_member, counts=None):
     """Reads the gzip file at `path` into pinned memory and decodes each member's DEFLATE body with the reader `d`
     (lb2_inflate_run), checking framing, CRC-32 and ISIZE; raises what gunzip raises.  After each member,
     on_member(isize, last, stats) is called while its bytes are still the reader's output (`last`: no member follows;
-    stats: its N.InflateStats).
+    stats: its N.InflateStats).  A file written with a seek table (seek_table.py) is decoded from the table
+    (lb2_inflate_run_table) and its table member is not a member here; counts (a dict, may be None) then gains
+    seek_table 1, or seek_table_refused 1 when the reader did not accept the table and searched instead.
     Returns (the first member's MTIME or None, the bytes uploaded)."""
     lib, h_in, mtime, uploaded = ctx.lib, None, None, 0
     try:
@@ -340,14 +396,24 @@ def inflate_members(ctx, d, path, on_member):
         with open(path, "rb") as f:
             if size and f.readinto(memoryview(buf).cast("B")) != size:
                 raise EOFError("%s changed while it was read" % path)
-        members = gzip_members(memoryview(buf).cast("B") if size else buf)
+        end, spans = _seek_spans(buf, size)
+        members = gzip_members(memoryview(buf).cast("B")[:end] if size else buf)
         body = next(members, None)
         if body is not None:
             start = next(i for i in range(size) if buf[i])
             mtime = struct.unpack_from("<I", buf, start + 4)[0]
         while body is not None:
             out_n, st = C.c_uint64(), N.InflateStats()
-            rc = lib.lb2_inflate_run(d, h_in + body, size - body, C.byref(out_n), C.byref(st))
+            if spans is not None:
+                used, refused = C.c_uint32(), C.c_uint32()
+                rc = lib.lb2_inflate_run_table(d, h_in + body, size - body, spans, len(spans), C.byref(out_n),
+                                               C.byref(st), C.byref(used), C.byref(refused))
+                if counts is not None:
+                    counts["seek_table"] = counts.get("seek_table", 0) + used.value
+                    counts["seek_table_refused"] = counts.get("seek_table_refused", 0) + refused.value
+                spans = None
+            else:
+                rc = lib.lb2_inflate_run(d, h_in + body, size - body, C.byref(out_n), C.byref(st))
             uploaded += size - body
             if rc == N.LB2_E_DATA:
                 raise InflateDataError("%s: %s" % (path, (lib.lb2_last_error(ctx.h) or b"").decode()))
@@ -362,9 +428,9 @@ def inflate_members(ctx, d, path, on_member):
             if want_isize != isize & 0xFFFFFFFF:
                 raise gzip.BadGzipFile("Incorrect length of data produced")
             k = t + 8
-            while k < size and buf[k] == 0:
+            while k < end and buf[k] == 0:
                 k += 1
-            on_member(isize, k >= size, st)
+            on_member(isize, k >= end, st)
             try:
                 body = members.send(st.in_bytes)
             except StopIteration:
@@ -463,7 +529,7 @@ class GpuTarReader:
                 ctx.d2d(self._arena + state["fill"], d_out.value, isize)
             state["fill"] = need
 
-        mtime, self.uploaded = inflate_members(ctx, self._d, path, on_member)
+        mtime, self.uploaded = inflate_members(ctx, self._d, path, on_member, self._stats)
         ref = state["ref"] or ((self._arena or 0), state["fill"])
         return ref, mtime
 
@@ -829,7 +895,7 @@ def strip_with(src, dst, reader, indexer, stripper, open_writer, piece_bytes=PIE
 
 
 def strip_tarball(src, dst, ctx=None, compresslevel=None, fallback_host_strip=True, tolerate_non_elf=False,
-                  piece_bytes=PIECE_BYTES):
+                  piece_bytes=PIECE_BYTES, seek_table=False):
     """Write `dst` as `src` (a .tar.gz) with every shared object stripped: the tar stream the reference's three passes
     (tarfile "r:gz" extract, `find -name "*.so" | xargs strip`, tarfile "w:gz") would write, without the tree.
 
@@ -844,7 +910,8 @@ def strip_tarball(src, dst, ctx=None, compresslevel=None, fallback_host_strip=Tr
     it; stripped data is zero-padded to 512 bytes; two zero blocks and zero padding to a multiple of RECORDSIZE end
     it, as TarFile.close() writes them; nothing after the source's end-of-archive marker is kept.  The gzip layer is
     one member with GpuGzipFile's header (MTIME from the source's first member) and the DEFLATE body GpuGzipFile
-    writes for that tar stream at the same compresslevel and piece_bytes.
+    writes for that tar stream at the same compresslevel and piece_bytes; seek_table=True appends GpuGzipFile's seek
+    table, so that dst reads back in one pass.  A source with a seek table is read from it.
 
     An ELF the planner refuses is fetched, stripped by the host `strip` and uploaded again (fallback_host_strip); a
     member `strip` refuses raises zipfile_gpu.StripFailed unless it is not an ELF and tolerate_non_elf keeps it.
@@ -864,7 +931,7 @@ def strip_tarball(src, dst, ctx=None, compresslevel=None, fallback_host_strip=Tr
 
     def open_writer(fileobj, name, mtime):
         return GpuGzipFile(name, mtime=mtime, ctx=ctx, piece_bytes=piece_bytes, compresslevel=compresslevel,
-                           fileobj=fileobj, host_buffers=False)
+                           fileobj=fileobj, host_buffers=False, seek_table=seek_table)
     try:
         with GpuTarReader(ctx) as reader, GpuStripper(ctx) as stripper:
             return strip_with(src, dst, reader, GpuTarIndex(ctx), stripper, open_writer, piece_bytes,
@@ -875,7 +942,7 @@ def strip_tarball(src, dst, ctx=None, compresslevel=None, fallback_host_strip=Tr
 
 
 def main(argv=None):
-    """python -m lambdipy_b200.tarball strip SRC DST [--level 9]"""
+    """python -m lambdipy_b200.tarball strip SRC DST [--level 9] [--seek-table]"""
     import argparse
     ap = argparse.ArgumentParser(prog="python -m lambdipy_b200.tarball")
     sub = ap.add_subparsers(dest="command", required=True)
@@ -883,8 +950,10 @@ def main(argv=None):
     sp.add_argument("src")
     sp.add_argument("dst")
     sp.add_argument("--level", type=int, choices=[9], default=None, help="9: the optimal parse (smaller, slower)")
+    sp.add_argument("--seek-table", action="store_true",
+                    help="append a seek table, with which the GPU reader decodes DST without searching for block starts")
     args = ap.parse_args(argv)
-    st = strip_tarball(args.src, args.dst, compresslevel=args.level)
+    st = strip_tarball(args.src, args.dst, compresslevel=args.level, **ST.seek_kw(args.seek_table))
     print("Tarball: %s, %.1f MB -> %.1f MB; %d shared objects stripped (%d via host strip), %.1f MB -> %.1f MB"
           % (args.dst, st["src_bytes"] / 1e6, st["dst_bytes"] / 1e6, st["gpu"] + st["fallback"], st["fallback"],
              st["in_bytes"] / 1e6, st["out_bytes"] / 1e6))

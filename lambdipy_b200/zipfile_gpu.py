@@ -43,6 +43,8 @@ import tempfile
 import zipfile
 
 from . import _native as N
+from . import seek_table as ST
+from .seek_table import seek_kw
 
 PIECE_BYTES = 64 << 20  # file bytes (and padding) per GPU submission
 MAX_SEGS = 1 << 16      # files per piece
@@ -59,9 +61,13 @@ class GpuZipEncoder:
     compresslevel: None (the default encoder) or 9 (the optimal parse, LB2_DEFLATE_BEST).
 
     submit_device(refs, flags) hands over a piece whose segments are (device address, length) pairs instead, laid out
-    by the library (lb2_zip_submit_device); a writer fed only that way needs no piece buffers (host_buffers=False)."""
+    by the library (lb2_zip_submit_device); a writer fed only that way needs no piece buffers (host_buffers=False).
 
-    def __init__(self, ctx, piece_bytes=PIECE_BYTES, max_segs=MAX_SEGS, compresslevel=None, host_buffers=True):
+    seek_table=True: after each collect(), seek_chunks holds every segment's [(compressed, decoded)] 64 KB chunks
+    (lb2_zip_chunk_sizes), from which the container writes each member's seek table (seek_table.py); else it is None."""
+
+    def __init__(self, ctx, piece_bytes=PIECE_BYTES, max_segs=MAX_SEGS, compresslevel=None, host_buffers=True,
+                 seek_table=False):
         flags = N.deflate_flags(compresslevel)  # checked before anything is allocated
         self._ctx, self._z, self._ptrs, self._out = ctx, None, [], None
         self.piece_bytes, self.max_segs = int(piece_bytes), int(max_segs)
@@ -79,14 +85,16 @@ class GpuZipEncoder:
         except BaseException:
             self.close()
             raise
-        self._pending = []  # segment count of each piece in flight
+        self._pending = []  # segment lengths of each piece in flight
         self._stats = N.GzipStats()
+        self._seek = bool(seek_table)
+        self.seek_chunks = None
 
     def submit(self, k, n, seg_off, seg_len, flags):
         ns = len(seg_off)
         offs, lens = (C.c_uint64 * ns)(*seg_off), (C.c_uint64 * ns)(*seg_len)
         self._ctx.check(self._ctx.lib.lb2_zip_submit(self._z, self._ptrs[k], n, offs, lens, ns, flags))
-        self._pending.append(ns)
+        self._pending.append(list(seg_len))
 
     def submit_device(self, refs, flags):
         ns = len(refs)
@@ -94,13 +102,27 @@ class GpuZipEncoder:
         for i, (addr, n) in enumerate(refs):
             src[i].d_ptr, src[i].len = addr, n
         self._ctx.check(self._ctx.lib.lb2_zip_submit_device(self._z, src, ns, flags))
-        self._pending.append(ns)
+        self._pending.append([n for _, n in refs])
 
     def collect(self):
-        ns = self._pending.pop(0)
+        lens = self._pending.pop(0)
+        ns = len(lens)
         segs, n = (N.ZipSegment * ns)(), C.c_uint64()
         self._ctx.check(self._ctx.lib.lb2_zip_collect(self._z, self._out, self._cap, C.byref(n), segs, C.byref(self._stats)))
         body = memoryview((C.c_uint8 * n.value).from_address(self._out)).cast("B") if n.value else memoryview(b"")
+        if self._seek:
+            counts = [max(1, -(-k // CHUNK)) for k in lens]
+            sizes, k = (C.c_uint32 * max(sum(counts), 1))(), C.c_uint32()
+            self._ctx.check(self._ctx.lib.lb2_zip_chunk_sizes(self._z, sizes, len(sizes), C.byref(k)))
+            if k.value != sum(counts):
+                raise RuntimeError("lb2_zip_chunk_sizes: %d chunks for %d" % (k.value, sum(counts)))
+            self.seek_chunks, at = [], 0
+            for seg, length, cnt in zip(segs, lens, counts):
+                ch = [(sizes[at + j], min(CHUNK, length - j * CHUNK)) for j in range(cnt)]
+                if sum(c for c, _ in ch) != seg.out_len:
+                    raise RuntimeError("lb2_zip_chunk_sizes: the chunks of a segment do not add up to its bytes")
+                self.seek_chunks.append(ch)
+                at += cnt
         return body, [(s.out_off, s.out_len, s.crc32, bool(s.ended)) for s in segs]
 
     def stats(self):
@@ -144,12 +166,13 @@ def tree_entries(root_dir):
     return entries
 
 
-def central_directory(infos, start, comment=b""):
+def central_directory(infos, start, comment=b"", tables=None):
     """The central directory of `infos` (written from offset `start`) and the end records, as ZipFile.close() writes
     them: zip64 extras for sizes or offsets beyond ZIP64_LIMIT, zip64 end records beyond 65 535 entries or 4 GiB, then
-    the archive comment."""
+    the archive comment.  tables {index: seek table}: appended to that entry's extra fields, either a member's
+    [(compressed, decoded)] chunks (seek_table.zip_field) or a field kept as it is."""
     out = []
-    for zi in infos:
+    for i, zi in enumerate(infos):
         dt = zi.date_time
         dosdate = (dt[0] - 1980) << 9 | dt[1] << 5 | dt[2]
         dostime = dt[3] << 11 | dt[4] << 5 | (dt[5] // 2)
@@ -169,6 +192,9 @@ def central_directory(infos, start, comment=b""):
             extra_data = zipfile._strip_extra(extra_data, (1,))
             extra_data = struct.pack("<HH" + "Q" * len(extra), 1, 8 * len(extra), *extra) + extra_data
             min_version = zipfile.ZIP64_VERSION
+        t = tables.get(i) if tables else None
+        if t is not None:
+            extra_data += t if isinstance(t, bytes) else ST.zip_field(t, len(extra_data))
         filename, flag_bits = zi._encodeFilenameFlags()
         out.append(struct.pack(zipfile.structCentralDir, zipfile.stringCentralDir, max(min_version, zi.create_version),
                                zi.create_system, max(min_version, zi.extract_version), zi.reserved, flag_bits,
@@ -191,11 +217,13 @@ class _ContainerWriter:
     a file's local header when its first body bytes arrive, rewritten with the CRC and sizes once it ends (seeking
     back, as ZipFile does on a seekable file).  With `copy` (strip_zip), an entry whose body never arrives is not a
     directory of the tree but a member kept as it is: copy(ZipInfo) writes its header and body at the current
-    position."""
+    position.  part(..., chunks) with every part's chunks gives the file a seek table in the central directory;
+    tables {entry index: table} are what central_directory writes."""
 
     def __init__(self, fp, entries, copy=None):
         self.fp, self.entries, self.next, self.copy = fp, entries, 0, copy
         self.cur = None  # (ZipInfo, zip64) of the file being written
+        self.tables = {}
         self.in_bytes = self.out_bytes = self.n_files = 0
 
     def _upto(self, idx):
@@ -210,7 +238,7 @@ class _ContainerWriter:
                 self.fp.write(zi.FileHeader(False))
             self.next += 1
 
-    def part(self, idx, body, crc, ended, file_bytes):
+    def part(self, idx, body, crc, ended, file_bytes, chunks=None):
         if self.cur is None:
             self._upto(idx)
             zi = self.entries[idx][1]
@@ -223,7 +251,9 @@ class _ContainerWriter:
             zi.header_offset = self.fp.tell()
             self.fp.write(zi.FileHeader(zip64))
             self.cur, self.cur_in, self.cur_out = (zi, zip64), 0, 0
+            self.cur_chunks = []
         self.fp.write(body)
+        self.cur_chunks = None if chunks is None or self.cur_chunks is None else self.cur_chunks + chunks
         self.cur_in += file_bytes
         self.cur_out += len(body)
         if ended:
@@ -238,13 +268,16 @@ class _ContainerWriter:
             self.in_bytes += self.cur_in
             self.out_bytes += self.cur_out
             self.n_files += 1
+            self.tables.pop(idx, None)
+            if self.cur_chunks:
+                self.tables[idx] = self.cur_chunks
             self.cur = None
             self.next = idx + 1
 
     def finish(self, comment=b""):
         self._upto(len(self.entries))
         start = self.fp.tell()
-        self.fp.write(central_directory([zi for _, zi in self.entries], start, comment))
+        self.fp.write(central_directory([zi for _, zi in self.entries], start, comment, self.tables))
 
 
 def _read_into(f, view):
@@ -274,8 +307,9 @@ def write_zip(root_dir, zip_path, encoder):
 
         def collect():
             body, res = encoder.collect()
-            for (idx, nbytes), (off, n, crc, ended) in zip(in_flight.pop(0), res):
-                w.part(idx, body[off:off + n], crc, ended, nbytes)
+            chunks = getattr(encoder, "seek_chunks", None) or [None] * len(res)
+            for (idx, nbytes), (off, n, crc, ended), ch in zip(in_flight.pop(0), res, chunks):
+                w.part(idx, body[off:off + n], crc, ended, nbytes, ch)
 
         def submit(more):
             nonlocal k, fill, segs, cont
@@ -319,21 +353,23 @@ def write_zip(root_dir, zip_path, encoder):
     return st
 
 
-def zip_tree(root_dir, zip_path, ctx=None, piece_bytes=PIECE_BYTES, compresslevel=None):
+def zip_tree(root_dir, zip_path, ctx=None, piece_bytes=PIECE_BYTES, compresslevel=None, seek_table=False):
     """Write `zip_path` as `shutil.make_archive(zip_path[:-4], "zip", root_dir)` would, with every member's DEFLATE
     body and CRC-32 computed on the GPU.  Returns a stats dict: files, entries, in_bytes (file bytes), out_bytes
     (member bodies), zip_bytes, kernel_ms (deflate + CRC-32 kernels, CUDA events), n_chunks, n_stored_chunks,
     n_fixed_chunks, n_opt_chunks and the copy times.  ctx=None: the context the strip path has already warmed up, if
     any, else a new one on device LAMBDIPY_B200_DEVICE (default 0).  compresslevel: None keeps the default encoder,
-    9 selects the optimal parse (smaller, slower); anything else raises ValueError.  There is no CPU path: without a
-    GPU this raises."""
+    9 selects the optimal parse (smaller, slower); anything else raises ValueError.  seek_table=True gives every
+    DEFLATE member of two or more 64 KB chunks a seek table in its central-directory entry (seek_table.py), with which
+    the GPU reader decodes it without searching for block starts; the archive up to the central directory is the one
+    written without.  There is no CPU path: without a GPU this raises."""
     from .tarball import _default_context
     N.deflate_flags(compresslevel)
     own = False
     if ctx is None:
         ctx, own = _default_context()
     try:
-        with GpuZipEncoder(ctx, piece_bytes, compresslevel=compresslevel) as enc:
+        with GpuZipEncoder(ctx, piece_bytes, compresslevel=compresslevel, seek_table=seek_table) as enc:
             return write_zip(root_dir, zip_path, enc)
     finally:
         if own:
@@ -397,14 +433,29 @@ class GpuUnzipDecoder:
         p = self._grow("_in", n)
         return memoryview((C.c_uint8 * n).from_address(p)).cast("B") if n else memoryview(bytearray())
 
-    def run(self, n, members, device=False):
+    def run(self, n, members, device=False, tables=None):
+        """tables (may be None): one seek table [(compressed, decoded)] or None per member (lb2_unzip_run_table)"""
         k = len(members)
         tab = (N.UnzipMember * max(k, 1))()
         for i, (off, blen, size, crc, method) in enumerate(members):
             tab[i].body_off, tab[i].body_len, tab[i].size, tab[i].crc32, tab[i].method = off, blen, size, crc, method
         res, out_n, st = (N.UnzipResult * max(k, 1))(), C.c_uint64(), N.UnzipStats()
         lib = self._ctx.lib
-        rc = lib.lb2_unzip_run(self._u, self._in if n else None, n, tab, k, C.byref(out_n), res, C.byref(st))
+        if tables:
+            first = (C.c_uint32 * (k + 1))()
+            flat = [e for t in tables for e in (t or [])]
+            spans = (N.InflateSpan * max(len(flat), 1))()
+            for i, t in enumerate(tables):
+                first[i + 1] = first[i] + len(t or [])
+            for i, (c, u) in enumerate(flat):
+                spans[i].in_len, spans[i].out_len = c, u
+            used, refused = C.c_uint32(), C.c_uint32()
+            rc = lib.lb2_unzip_run_table(self._u, self._in if n else None, n, tab, k, first, spans, C.byref(out_n), res,
+                                         C.byref(st), C.byref(used), C.byref(refused))
+            self._stats["seek_table"] = self._stats.get("seek_table", 0) + used.value
+            self._stats["seek_table_refused"] = self._stats.get("seek_table_refused", 0) + refused.value
+        else:
+            rc = lib.lb2_unzip_run(self._u, self._in if n else None, n, tab, k, C.byref(out_n), res, C.byref(st))
         if rc == N.LB2_E_CAPACITY:
             raise DeviceTooSmall((lib.lb2_last_error(self._ctx.h) or b"").decode())
         self._ctx.check(rc)
@@ -419,10 +470,10 @@ class GpuUnzipDecoder:
         out = memoryview((C.c_uint8 * out_n.value).from_address(p)).cast("B") if out_n.value else memoryview(b"")
         return [(res[i].status, out[res[i].out_off:res[i].out_off + members[i][2]]) for i in range(k)]
 
-    def run_device(self, n, members):
+    def run_device(self, n, members, tables=None):
         """run() with the decoded members left on the device: [(status, (device address, size))], the addresses
         multiples of 16 inside one buffer and valid until the next run."""
-        return self.run(n, members, device=True)
+        return self.run(n, members, device=True, tables=tables)
 
     def stats(self):
         d = dict(self._stats)
@@ -539,7 +590,7 @@ class _Reader:
         buf = self.decoder.buffer(max(hi - lo, 0))
         self.fp.seek(lo)
         _read_into(self.fp, buf)
-        members, infos = [], []
+        members, infos, tables = [], [], []
         for zi in todo:
             b = _body(self.zf, zi, buf, lo, self.archive_bytes)
             if b is not None and b[1] < 0:
@@ -547,8 +598,10 @@ class _Reader:
             elif b is not None:
                 members.append((b[0], b[1], zi.file_size, zi.CRC, zi.compress_type))
                 infos.append(zi)
+                tables.append(_seek_entries(zi))
         try:
-            res = self.decoder.run(len(buf), members)
+            res = self.decoder.run(len(buf), members, tables=tables) if any(tables) else \
+                self.decoder.run(len(buf), members)
         except DeviceTooSmall:
             if len(infos) == 1:
                 return  # does not fit on the device alone: the stdlib's code reads it
@@ -567,6 +620,14 @@ class _Reader:
               "out_bytes": self.out_bytes}
         st.update(self.decoder.stats())
         return st
+
+
+def _seek_entries(zi):
+    """the seek table of a DEFLATE member from its central-directory extra field, or None (none, or not valid)"""
+    if zi.compress_type != zipfile.ZIP_DEFLATED:
+        return None
+    entries = ST.zip_entries(zi.extra)
+    return entries if ST.valid(entries, zi.compress_size, zi.file_size) else None
 
 
 def _raise_for(zi, status):
@@ -792,10 +853,11 @@ def selected_for_strip(zi):
 
 def _kept(zi):
     """A copy of a source archive's ZipInfo for the archive being written: no data descriptor (the sizes are known),
-    no zip64 extra field (FileHeader and central_directory make their own)."""
+    no zip64 extra field (FileHeader and central_directory make their own), no seek table (it belongs in the central
+    directory only: strip_with hands it to the writer's tables)."""
     out = copy.copy(zi)
     out.flag_bits &= ~zipfile._MASK_USE_DATA_DESCRIPTOR
-    out.extra = zipfile._strip_extra(zi.extra, (1,))
+    out.extra = zipfile._strip_extra(zi.extra, (1, ST.ZIP_ID))
     return out
 
 
@@ -868,13 +930,18 @@ def strip_with(src_zip, dst_zip, decoder, stripper, encoder, fallback_host_strip
                     left -= len(block)
 
             w = _ContainerWriter(fp, entries, copy=copy_member)
+            for idx, zi in enumerate(zf.filelist):   # a member copied as it is keeps its seek table
+                field = ST.zip_field_of(zi.extra)
+                if field:
+                    w.tables[idx] = field
             in_flight = []
 
             def collect():
                 body, res = encoder.collect()
                 n["downloaded"] += len(body)
-                for (idx, (_, nbytes)), (off, k, crc, ended) in zip(in_flight.pop(0), res):
-                    w.part(idx, body[off:off + k], crc, ended, nbytes)
+                chunks = getattr(encoder, "seek_chunks", None) or [None] * len(res)
+                for (idx, (_, nbytes)), (off, k, crc, ended), ch in zip(in_flight.pop(0), res, chunks):
+                    w.part(idx, body[off:off + k], crc, ended, nbytes, ch)
 
             def host_path(idx, zi, data):
                 """the stripped bytes of a member the device did not strip, on the device; None: keep the member"""
@@ -891,7 +958,7 @@ def strip_with(src_zip, dst_zip, decoder, stripper, encoder, fallback_host_strip
             def run(batch):
                 """batch: [(entry index, source ZipInfo)] of selected members, in archive order"""
                 view = decoder.buffer(sum(zi.compress_size for _, zi in batch))
-                members, taken, fill = [], [], 0
+                members, taken, tables, fill = [], [], [], 0
                 for idx, zi in batch:
                     if not _gpu_member(zi):
                         continue
@@ -907,11 +974,14 @@ def strip_with(src_zip, dst_zip, decoder, stripper, encoder, fallback_host_strip
                         raise BadZipMember(zi.filename, "The archive ends inside the body")
                     members.append((fill, zi.compress_size, zi.file_size, zi.CRC, zi.compress_type))
                     taken.append(idx)
+                    tables.append(_seek_entries(zi))
                     fill += zi.compress_size
                 decoded = {}
                 try:
                     if taken:
-                        decoded = dict(zip(taken, decoder.run_device(fill, members)))
+                        res = decoder.run_device(fill, members, tables=tables) if any(tables) else \
+                            decoder.run_device(fill, members)
+                        decoded = dict(zip(taken, res))
                         n["uploaded"] += fill
                 except DeviceTooSmall:
                     if len(taken) > 1:
@@ -988,7 +1058,7 @@ def _umask():
 
 
 def strip_zip(src_zip, dst_zip, ctx=None, compresslevel=None, fallback_host_strip=True, tolerate_non_elf=False,
-              batch_bytes=BATCH_BYTES, piece_bytes=PIECE_BYTES):
+              batch_bytes=BATCH_BYTES, piece_bytes=PIECE_BYTES, seek_table=False):
     """Write `dst_zip` with the members of `src_zip`, in their order, every `*.so` member stripped: the archive that
     `ZipFile(src_zip).extractall(d)`, the reference's `find d/ -name "*.so" | xargs strip` and a zip of `d` lead to,
     without the tree.  src_zip is only read; dst_zip appears under its name when it is complete, and not at all when
@@ -1006,7 +1076,9 @@ def strip_zip(src_zip, dst_zip, ctx=None, compresslevel=None, fallback_host_stri
     in strip_tree; so is a selected member the GPU reader does not take (encrypted, bzip2 ...: the stdlib reads it
     and raises what it raises).  A member `strip` refuses raises StripFailed -- the reference's xargs exits 123 --
     unless it is not an ELF and tolerate_non_elf keeps it as it is.  A member that does not read back raises
-    BadZipMember.  compresslevel: None or 9, as zip_tree.
+    BadZipMember.  compresslevel: None or 9, as zip_tree.  A source member's seek table is used to read it; a member
+    copied as it is keeps its table in the central directory, a rewritten one drops it and, with seek_table=True,
+    gets a new one, as zip_tree writes it.
 
     Returns a stats dict: members, selected, gpu, fallback, skipped; in_bytes / out_bytes (the stripped members
     before and after) and deflated_bytes (their new bodies); src_zip_bytes, zip_bytes; uploaded_bytes,
@@ -1020,7 +1092,7 @@ def strip_zip(src_zip, dst_zip, ctx=None, compresslevel=None, fallback_host_stri
         ctx, own = _default_context()
     try:
         with GpuUnzipDecoder(ctx) as dec, GpuStripper(ctx) as stripper, \
-                GpuZipEncoder(ctx, piece_bytes, compresslevel=compresslevel, host_buffers=False) as enc:
+                GpuZipEncoder(ctx, piece_bytes, compresslevel=compresslevel, host_buffers=False, seek_table=seek_table) as enc:
             return strip_with(src_zip, dst_zip, dec, stripper, enc, fallback_host_strip, tolerate_non_elf, batch_bytes)
     finally:
         if own:
@@ -1028,7 +1100,7 @@ def strip_zip(src_zip, dst_zip, ctx=None, compresslevel=None, fallback_host_stri
 
 
 def main(argv=None):
-    """python -m lambdipy_b200.zipfile_gpu strip SRC DST [--level 9]"""
+    """python -m lambdipy_b200.zipfile_gpu strip SRC DST [--level 9] [--seek-table]"""
     import argparse
     from . import patch, project_build
     ap = argparse.ArgumentParser(prog="python -m lambdipy_b200.zipfile_gpu")
@@ -1037,8 +1109,10 @@ def main(argv=None):
     sp.add_argument("src")
     sp.add_argument("dst")
     sp.add_argument("--level", type=int, choices=[9], default=None, help="9: the optimal parse (smaller, slower)")
+    sp.add_argument("--seek-table", action="store_true",
+                    help="give the rewritten members seek tables, with which the GPU reader decodes them without search")
     args = ap.parse_args(argv)
-    st = strip_zip(args.src, args.dst, compresslevel=args.level)
+    st = strip_zip(args.src, args.dst, compresslevel=args.level, **seek_kw(args.seek_table))
     with zipfile.ZipFile(args.dst) as zf:
         unzipped = sum(zi.file_size for zi in zf.filelist)
     print("Bundle zip: %s, %.1f MB = %.0f %% of the 50 MB direct-upload limit; unzipped %.1f MB = %.0f %% of 250 MB; "
