@@ -15,6 +15,8 @@ Public surface:
                                                 archive), every member's DEFLATE body compressed on the GPU
     extract_zip(zip_path, directory)            ZipFile.extractall's tree, every member inflated on the GPU
     testzip(zip_path)                           ZipFile.testzip's answer, every member checked on the GPU
+    zip_tarballs(srcs, dst, prefix="")          the Lambda zip of .tar.gz package assets, shared objects stripped,
+                                                inflated, stripped and deflated on the GPU without unpacking them
     patch.apply()                               monkey-patch an installed lambdipy in place
 The byte work is done by liblambdipy_b200.so (CUDA, C ABI in include/lambdipy_b200.h).
 """
@@ -31,4 +33,7 @@ def __getattr__(name):
     if name in ("zip_tree", "extract_zip", "testzip"):
         from . import zipfile_gpu
         return getattr(zipfile_gpu, name)
+    if name == "zip_tarballs":
+        from . import layer
+        return layer.zip_tarballs
     raise AttributeError(name)

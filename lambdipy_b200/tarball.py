@@ -503,9 +503,10 @@ class GpuTarReader:
         except N.NativeError as e:
             raise N.NativeError(N.LB2_E_CAPACITY, "the tar stream does not fit in device memory (%s)" % e) from None
 
-    def read(self, path):
+    def _decode(self, path, state, in_place):
+        """inflate_members on `path`, every member appended to the arena at state["fill"]; in_place: a file of one
+        member is left in the reader's output buffer instead and state["ref"] is set to it.  Returns the MTIME."""
         ctx, lib = self._ctx, self._ctx.lib
-        state = {"ref": None, "fill": 0, "cap": 0}
 
         def on_member(isize, last, st):
             for k, v in st.as_dict().items():
@@ -513,12 +514,12 @@ class GpuTarReader:
                     self._stats[k] = self._stats.get(k, 0) + v
             d_out, n = C.c_void_p(), C.c_uint64()
             ctx.check(lib.lb2_inflate_device_output(self._d, C.byref(d_out), C.byref(n)))
-            if state["ref"] is None and state["fill"] == 0 and last:
+            if in_place and state["ref"] is None and state["fill"] == 0 and last:
                 state["ref"] = (d_out.value or 0, n.value)    # the only member: used where it lies
                 return
             need = state["fill"] + isize
             if need > state["cap"]:
-                cap = max(need, 2 * state["cap"], 1 << 20)
+                cap = -(-max(need, 2 * state["cap"], 1 << 20) // 256) * 256   # read_many's next start stays inside
                 arena = self._alloc(cap)
                 if state["fill"]:
                     ctx.d2d(arena, self._arena, state["fill"])
@@ -529,9 +530,29 @@ class GpuTarReader:
                 ctx.d2d(self._arena + state["fill"], d_out.value, isize)
             state["fill"] = need
 
-        mtime, self.uploaded = inflate_members(ctx, self._d, path, on_member, self._stats)
+        mtime, uploaded = inflate_members(ctx, self._d, path, on_member, self._stats)
+        self.uploaded += uploaded
+        return mtime
+
+    def read(self, path):
+        state = {"ref": None, "fill": 0, "cap": 0}
+        self.uploaded = 0
+        mtime = self._decode(path, state, True)
         ref = state["ref"] or ((self._arena or 0), state["fill"])
         return ref, mtime
+
+    def read_many(self, paths):
+        """The tar streams of several gzip files in one device arena, each at a 256-byte-aligned offset: [(address,
+        length)] in the order of `paths`, valid until close().  One file is read() as it is."""
+        if len(paths) == 1:
+            return [self.read(paths[0])[0]]
+        state, spans = {"ref": None, "fill": 0, "cap": 0}, []
+        self.uploaded = 0
+        for path in paths:
+            state["fill"] = start = -(-state["fill"] // 256) * 256
+            self._decode(path, state, False)
+            spans.append((start, state["fill"] - start))
+        return [((self._arena or 0) + off, n) for off, n in spans]   # the arena moves while it grows
 
     def fetch(self, addr, n):
         buf = C.create_string_buffer(n)
@@ -639,6 +660,18 @@ class IndexedView:
             self.miss_bytes += end - pos
         self._pos = end
         return out
+
+
+def list_members(ref, indexer, reader):
+    """tarfile's member list of the tar stream at ref = (address, length) in device memory, read from one index
+    download: (members, the offset tarfile stopped at, the IndexedView, (ranges, their bytes, the index's stats))."""
+    base, n = ref
+    ranges, data, ist = indexer.index(ref)
+    view = IndexedView(n, ranges, data, lambda off, k: reader.fetch(base + off, k))
+    with tarfile.open(fileobj=view, mode="r:") as tar:
+        members = tar.getmembers()
+        stop = tar.offset
+    return members, stop, view, (ranges, data, ist)
 
 
 def _norm(name):
@@ -811,11 +844,7 @@ def strip_with(src, dst, reader, indexer, stripper, open_writer, piece_bytes=PIE
     try:
         with os.fdopen(fd, "wb") as fp:
             (base, n), mtime = reader.read(src)
-            ranges, data, ist = indexer.index((base, n))
-            view = IndexedView(n, ranges, data, lambda off, k: reader.fetch(base + off, k))
-            with tarfile.open(fileobj=view, mode="r:") as tar:
-                members = tar.getmembers()
-                stop = tar.offset
+            members, stop, view, (ranges, data, ist) = list_members((base, n), indexer, reader)
             chosen, skipped = select_members(members)
             res = stripper.strip([(base + members[i].offset_data, members[i].size) for i in chosen]) if chosen else []
             new, c = {}, {"gpu": 0, "fallback": 0, "skipped": skipped, "in_bytes": 0, "out_bytes": 0}
