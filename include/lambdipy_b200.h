@@ -187,6 +187,9 @@ int lb2_strip_tree_ex(lb2_ctx *ctx, const char *root, const char *suffix, uint32
                       lb2_tree_stats *stats);
 /* Only the clean-up lines (no GPU, no context needed). */
 int lb2_tree_cleanup(const char *root, const char *keep_tests_regex, uint32_t *n_removed);
+/* The `tests` line of the clean-up on paths that are not on disk: removed[i] = 1 when an entry named tests that find
+ * prints as lines[i] is removed, 0 when the keep pattern keeps it.  The same rule lb2_tree_cleanup applies. */
+int lb2_cleanup_tests_removed(const char *keep_tests_regex, const char *const *lines, uint32_t n, uint8_t *removed);
 /* Optional: pay lb2_strip_tree's first-use costs (pinned slot ring, I/O streams, device workspaces) now,
  * e.g. on a helper thread while the reference's script is still running pip
  * (/root/reference/lambdipy/project_build.py:266-268).  expected_tree_bytes sizes the ring (0 = default). */

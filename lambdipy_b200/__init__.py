@@ -17,6 +17,8 @@ Public surface:
     testzip(zip_path)                           ZipFile.testzip's answer, every member checked on the GPU
     zip_tarballs(srcs, dst, prefix="")          the Lambda zip of .tar.gz package assets, shared objects stripped,
                                                 inflated, stripped and deflated on the GPU without unpacking them
+    zip_build(dst, tarballs, wheels)            the Lambda zip of a whole build: tarballs and wheels, pip's target
+                                                install and the build script's clean-up restated, strip on the GPU
     patch.apply()                               monkey-patch an installed lambdipy in place
 The byte work is done by liblambdipy_b200.so (CUDA, C ABI in include/lambdipy_b200.h).
 """
@@ -33,7 +35,7 @@ def __getattr__(name):
     if name in ("zip_tree", "extract_zip", "testzip"):
         from . import zipfile_gpu
         return getattr(zipfile_gpu, name)
-    if name == "zip_tarballs":
+    if name in ("zip_tarballs", "zip_build"):
         from . import layer
-        return layer.zip_tarballs
+        return getattr(layer, name)
     raise AttributeError(name)

@@ -31,6 +31,7 @@ EXPORTS = [
     "lb2_zip_submit_device", "lb2_unzip_device_output",
     "lb2_inflate_device_output", "lb2_memcpy_d2d", "lb2_gzip_submit_device", "lb2_tar_index",
     "lb2_gzip_chunk_sizes", "lb2_inflate_run_table", "lb2_zip_chunk_sizes", "lb2_unzip_run_table",
+    "lb2_cleanup_tests_removed",
 ]
 TAR_STOP_ZERO, TAR_STOP_BAD_HEADER, TAR_STOP_END, TAR_STOP_UNSUPPORTED = 1, 2, 3, 4
 ZIP_CONTINUES, ZIP_MORE = 1, 2
@@ -227,6 +228,8 @@ def load():
     lib.lb2_strip_tree_ex.restype = C.c_int
     lib.lb2_tree_cleanup.argtypes = [C.c_char_p, C.c_char_p, C.POINTER(C.c_uint32)]
     lib.lb2_tree_cleanup.restype = C.c_int
+    lib.lb2_cleanup_tests_removed.argtypes = [C.c_char_p, C.POINTER(C.c_char_p), C.c_uint32, C.POINTER(C.c_uint8)]
+    lib.lb2_cleanup_tests_removed.restype = C.c_int
     lib.lb2_tree_prepare.argtypes = [vp, C.c_uint64]
     lib.lb2_tree_prepare.restype = C.c_int
     lib.lb2_gzip_create.argtypes = [vp, C.c_uint32, C.POINTER(vp)]

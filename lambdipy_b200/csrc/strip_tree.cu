@@ -41,6 +41,20 @@ struct Cleanup {
   ~Cleanup() { if (have_keep) regfree(&keep); }
 };
 
+// The `tests` line on one entry named tests: `line` is the path find prints for it.  grep reads the printed list line
+// by line, so a path holding a newline never matches as a whole and is left alone.
+static bool tests_removed(const Cleanup &cl, const std::string &line) {
+  return line.find('\n') == std::string::npos && !(cl.have_keep && regexec(&cl.keep, line.c_str(), 0, nullptr, 0) == 0);
+}
+
+static int compile_keep(Cleanup &cl, const char *keep_regex, std::string *err) {
+  if (keep_regex && *keep_regex) {
+    if (regcomp(&cl.keep, keep_regex, REG_NOSUB) != 0) { if (err) *err = std::string("bad keep-tests pattern: ") + keep_regex; return LB2_E_ARG; }
+    cl.have_keep = true;
+  }
+  return LB2_OK;
+}
+
 static void rm_rf(const std::string &p) {
   struct stat sb;
   if (lstat(p.c_str(), &sb) != 0) return;
@@ -85,8 +99,7 @@ static void walk(const std::string &dir, const std::string &shown, bool top, con
       bool remove = false;
       if (top && name[0] != '.' && (ends_with(name.c_str(), ".egg-info") || ends_with(name.c_str(), ".dist-info"))) remove = true;
       else if (name == "__pycache__") remove = true;
-      else if (name == "tests" && line.find('\n') == std::string::npos &&
-               !(cl->have_keep && regexec(&cl->keep, line.c_str(), 0, nullptr, 0) == 0)) remove = true;
+      else if (name == "tests" && tests_removed(*cl, line)) remove = true;
       if (remove) { rm_rf(p); cl->n_removed++; continue; }
     }
     if (suffix && ends_with(name.c_str(), suffix)) {
@@ -113,10 +126,7 @@ static int walk_root(const char *root, const char *suffix, bool cleanup, const c
   Cleanup cl;
   if (cleanup) {
     cl.on = true;
-    if (keep_regex && *keep_regex) {
-      if (regcomp(&cl.keep, keep_regex, REG_NOSUB) != 0) { if (err) *err = std::string("bad keep-tests pattern: ") + keep_regex; return LB2_E_ARG; }
-      cl.have_keep = true;
-    }
+    if (int rc = compile_keep(cl, keep_regex, err)) return rc;
   }
   walk(r, r + "/", true, suffix, &cl, files, st);
   st->n_removed = cl.n_removed;
@@ -281,6 +291,17 @@ int lb2_tree_cleanup(const char *root, const char *keep_tests_regex, uint32_t *n
   int rc = walk_root(root, nullptr, true, keep_tests_regex, nullptr, files, &st);
   if (rc) return rc;
   if (n_removed) *n_removed = st.n_removed;
+  return LB2_OK;
+}
+
+int lb2_cleanup_tests_removed(const char *keep_tests_regex, const char *const *lines, uint32_t n, uint8_t *removed) {
+  if (n && (!lines || !removed)) return LB2_E_ARG;
+  Cleanup cl;
+  if (int rc = compile_keep(cl, keep_tests_regex, nullptr)) return rc;
+  for (uint32_t i = 0; i < n; i++) {
+    if (!lines[i]) return LB2_E_ARG;
+    removed[i] = tests_removed(cl, lines[i]) ? 1 : 0;
+  }
   return LB2_OK;
 }
 

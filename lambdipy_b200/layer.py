@@ -19,14 +19,27 @@ the host `strip` fallback handles.
 
     zip_tarballs(srcs, dst, prefix="")
     python -m lambdipy_b200.layer DST SRC [SRC ...] [--prefix python/] [--level 9] [--seek-table]
+
+zip_build adds wheels to the same chain: pip's `--target` install and the build script's clean-up lines are restated
+on the merged tree, the wheels' shared objects are inflated on the GPU next to the tarballs' files, and every other
+wheel member's DEFLATE body is copied into the zip as it is.
+
+    zip_build(dst, tarballs=(), wheels=(), prefix="", keep_tests=())
+    python -m lambdipy_b200.layer DST [SRC ...] --wheel WHL [--wheel WHL ...] [--keep-tests NAME] [--clean]
 """
+import ctypes as C
+import email.parser
+import importlib.metadata
 import os
 import posixpath
+import re
 import stat
+import struct
 import sys
 import tempfile
 import time
 import zipfile
+import zlib
 
 from . import _native as N
 from . import seek_table as ST
@@ -49,6 +62,13 @@ class _File:
 
     def __init__(self):
         self.src, self.member, self.mode, self.mtime, self.links = None, None, 0, 0, 1
+
+    def position(self):
+        """where the file's data lies among the sources: the order the stripper takes it in"""
+        return self.src, self.member.offset_data
+
+    def label(self):
+        return self.member.name
 
 
 class _Link:
@@ -193,7 +213,7 @@ def select(nodes):
                 chosen.setdefault(id(t), t)
             else:
                 skipped += 1
-    return sorted(chosen.values(), key=lambda f: (f.src, f.member.offset_data)), skipped
+    return sorted(chosen.values(), key=lambda f: f.position()), skipped
 
 
 def zip_info(path, node, size, umask):
@@ -376,19 +396,623 @@ def zip_tarballs(srcs, dst, prefix="", ctx=None, compresslevel=None, fallback_ho
             ctx.close()
 
 
+# ---- zip_build: prebuilt tarballs and wheels, pip's target install and the build script's clean-up ----------------
+# pip is not run.  What `pip install --no-deps --no-index --target T W1.whl ...` (pip 24) does to the tree is restated
+# on the merged tree's nodes: every wheel is installed into a temporary home H (the scheme get_scheme(name, home=H)
+# gives), then the top-level items of H/lib/python and of H are moved into T as commands/install.py's
+# _handle_target_dir moves them.  Only the parts of pip that decide names, bytes and modes are restated; the RECORD,
+# INSTALLER, REQUESTED and direct_url.json files pip writes go with the .dist-info directory the clean-up removes.
+
+_WHEEL_FILE = re.compile(r"^(?P<name>[^\s-]+?)-(?P<ver>[^\s-]*?)(-(?P<build>\d[^-]*?))?-(?P<pyver>[^\s-]+?)"
+                         r"-(?P<abi>[^\s-]+?)-(?P<plat>[^\s-]+?)\.whl$")   # pip's Wheel.wheel_file_re
+_ENTRY = re.compile(r"(?P<name>([^\[]\S*))\s*=\s*(?P<callable>(\w+)([:\.]\w+)*)"
+                    r"\s*(\[\s*(?P<flags>[\w-]+(=\w+)?(,\s*\w+(=\w+)?)*)\s*\])?")   # distlib's ENTRY_RE
+_LAUNCHER = r"""# -*- coding: utf-8 -*-
+import re
+import sys
+from %(module)s import %(import_name)s
+if __name__ == '__main__':
+    sys.argv[0] = re.sub(r'(-script\.pyw|\.exe)?$', '', sys.argv[0])
+    sys.exit(%(func)s())
+"""                                                                   # distlib's SCRIPT_TEMPLATE, as pip 24 writes it
+_LIB = "lib/python"                                                   # purelib and platlib under the home
+BUILD_DIR = "./build/"   # the directory the reference's clean-up lines print paths under (`find ./build/ -name tests`)
+
+
+class _WheelFile(_File):
+    """a file pip installs: a wheel member (data None: its body is copied or decoded) or bytes made on the host (a
+    `#!python` script fixed, a console or gui script generated); date_time is the entry's"""
+
+    def __init__(self, src, member, mode, date_time, data=None):
+        super().__init__()
+        self.src, self.member, self.mode, self.date_time, self.data = src, member, mode, date_time, data
+
+    def position(self):
+        return self.src, self.member.header_offset if self.data is None else 1 << 62
+
+    def label(self):
+        return self.member.filename if self.member is not None else "a generated script"
+
+    def signature(self):
+        if self.data is not None:
+            return len(self.data), zlib.crc32(self.data), self.mode
+        return self.member.file_size, self.member.CRC, self.mode
+
+
+def canonical_name(name):
+    return re.sub(r"[-_.]+", "-", name).lower()
+
+
+def _shebang(executable):
+    """distlib's shebang for pip's console and gui scripts: the interpreter quoted when it holds a space, and the
+    /bin/sh trampoline when the line would hold a space or pass 127 bytes"""
+    if " " in executable and not executable.startswith('"'):
+        if executable.startswith("/usr/bin/env "):
+            env, rest = executable.split(" ", 1)
+            if " " in rest and not rest.startswith('"'):
+                executable = '%s "%s"' % (env, rest)
+        else:
+            executable = '"%s"' % executable
+    exe = executable.encode("utf-8")
+    if b" " not in exe and len(exe) + 3 <= 127:
+        return b"#!" + exe + b"\n"
+    return b"#!/bin/sh\n'''exec' " + exe + b' "$0" "$@"\n' + b"' '''\n"
+
+
+class _WheelMetadata(importlib.metadata.Distribution):
+    """the wheel's .dist-info read from the archive, for its entry points as pip's importlib backend reads them"""
+
+    def __init__(self, zf, info_dir):
+        self._zf, self._info = zf, info_dir
+
+    def read_text(self, filename):
+        try:
+            return self._zf.read(self._info + "/" + filename).decode("utf-8")
+        except KeyError:
+            return None
+
+    def locate_file(self, path):
+        raise NotImplementedError
+
+
+def read_wheel(path, src, umask, executable=sys.executable):
+    """(canonical name, {path under the temporary home: _WheelFile}) of what pip 24 installs from one wheel, checked
+    before anything is written: ValueError for a name that is not a wheel's, not exactly one .dist-info directory, a
+    Wheel-Version other than 1.x, a member leaving its scheme directory or under an unknown scheme key, a member that is
+    encrypted or compressed with anything but stored or deflated, an entry point without a callable, and the entry
+    points pip treats specially (pip, easy_install)."""
+    m = _WHEEL_FILE.match(os.path.basename(path))
+    if not m:
+        raise ValueError("%s: not a wheel file name (name-version-python-abi-platform.whl)" % path)
+    name = m.group("name").replace("_", "-")
+    with zipfile.ZipFile(path) as zf:
+        names = list(dict.fromkeys(zf.namelist()))     # a repeated name installs its last entry, as getinfo reads it
+        info_dirs = sorted({n.split("/", 1)[0] for n in names if n.split("/", 1)[0].endswith(".dist-info")})
+        if len(info_dirs) != 1:
+            raise ValueError("%s: %d .dist-info directories, one is needed" % (path, len(info_dirs)))
+        info_dir = info_dirs[0]
+        if not canonical_name(info_dir).startswith(canonical_name(name)):
+            raise ValueError("%s: .dist-info directory %r does not start with %r" % (path, info_dir, name))
+        try:
+            version = email.parser.Parser().parsestr(zf.read(info_dir + "/WHEEL").decode("utf-8"))["Wheel-Version"]
+            major = int(version.strip().split(".")[0])
+        except (KeyError, AttributeError, ValueError, UnicodeDecodeError):
+            raise ValueError("%s: no valid Wheel-Version in %s/WHEEL" % (path, info_dir)) from None
+        if major != 1:
+            raise ValueError("%s: Wheel-Version %s, only 1.x is supported" % (path, version.strip()))
+        scheme = {"purelib": _LIB, "platlib": _LIB, "scripts": "bin", "data": "",
+                  "headers": "include/site/python%d.%d/%s" % (sys.version_info[0], sys.version_info[1], name)}
+        meta = _WheelMetadata(zf, info_dir)
+        eps = meta.entry_points
+        console = {e.name: e.value for e in eps if e.group == "console_scripts"}
+        gui = {e.name: e.value for e in eps if e.group == "gui_scripts"}
+        if "pip" in console or "easy_install" in console:
+            raise ValueError("%s: the entry points pip installs itself under several names are not supported" % path)
+
+        def wrapper(base):
+            low = base.lower()
+            for suffix in (".exe", "-script.py", ".pya"):
+                if low.endswith(suffix):
+                    base = base[:-len(suffix)]
+                    break
+            return base in console or base in gui
+
+        files = {}
+        for n in names:
+            if n.endswith("/"):
+                continue
+            zi = zf.getinfo(n)
+            if zi.compress_type not in (zipfile.ZIP_STORED, zipfile.ZIP_DEFLATED) or zi.flag_bits & 0x1:
+                raise ValueError("%s: member %r is encrypted or compressed with method %d; only stored and deflated "
+                                 "members are read" % (path, n, zi.compress_type))
+            normed = posixpath.normpath(n)
+            if n.split("/", 1)[0].endswith(".data"):
+                parts = normed.split("/", 2)
+                if len(parts) < 3 or parts[1] not in scheme:
+                    raise ValueError("%s: member %r is not under <name>.data/<scheme key>/ (purelib, platlib, "
+                                     "headers, scripts, data)" % (path, n))
+                key, rel = parts[1], parts[2]
+            else:
+                key, rel = "purelib", normed
+            if T._leaves(rel) or rel in (".", ""):
+                raise ValueError("%s: member %r leaves the directory it is installed to" % (path, n))
+            dest = posixpath.join(scheme[key], rel) if scheme[key] else rel
+            mode = stat.S_IMODE(zi.external_attr >> 16)
+            executable_bit = bool(zi.external_attr >> 16 and stat.S_ISREG(zi.external_attr >> 16) and mode & 0o111)
+            mode = 0o777 & ~umask | 0o111 if executable_bit else 0o666 & ~umask
+            data = None
+            parts = n.split("/", 2)
+            if len(parts) > 2 and parts[0].endswith(".data") and parts[1] == "scripts":
+                if wrapper(posixpath.basename(dest)):
+                    continue                                  # the generated script takes its place
+                body = zf.read(zi)
+                first, nl, rest = body.partition(b"\n")
+                if first.startswith(b"#!python"):             # pip's fix_script
+                    data = b"#!" + os.fsencode(executable) + os.linesep.encode("ascii") + rest
+            files[dest] = _WheelFile(src, zi, mode, zi.date_time, data)
+        specs = [("%s = %s" % kv, False) for kv in console.items()] + [("%s = %s" % kv, True) for kv in gui.items()]
+        when = zf.getinfo(info_dir + "/entry_points.txt").date_time if specs else None
+        for spec, _ in specs:
+            e = _ENTRY.search(spec)
+            if not e or e.group("callable").count(":") != 1:
+                raise ValueError("%s: entry point %r has no callable (module:function)" % (path, spec))
+            module, func = e.group("callable").split(":")
+            text = _shebang(executable) + (_LAUNCHER % {"module": module, "import_name": func.split(".")[0],
+                                                         "func": func}).encode("utf-8")
+            dest = "bin/" + e.group("name")
+            if dest in files:
+                raise ValueError("%s: entry point %r would overwrite a file of the wheel" % (path, e.group("name")))
+            files[dest] = _WheelFile(src, None, 0o666 & ~umask | 0o555, when, text)
+    return canonical_name(name), files
+
+
+def read_home(wheels, umask=0o022, executable=sys.executable, first_src=0):
+    """The temporary home `pip install --no-deps --no-index --target` installs the wheels into, before anything moves:
+    ({path under the home: _WheelFile}, the number of scripts generated).  Two wheels may install the same path only
+    with the same size, CRC-32 and mode (the first wheel's entry is kept); any other overlap, one distribution given
+    twice and a path installed both as a file and as a directory raise ValueError, as read_wheel's refusals do."""
+    home, seen, generated = {}, {}, 0
+    for i, path in enumerate(wheels):
+        name, files = read_wheel(path, first_src + i, umask, executable)
+        if name in seen:
+            raise ValueError("%s and %s install the same distribution %r" % (wheels[seen[name]], path, name))
+        seen[name] = i
+        generated += sum(1 for f in files.values() if f.member is None)
+        for dest, f in files.items():
+            old = home.get(dest)
+            if old is not None and old.signature() != f.signature():
+                raise ValueError("%s and %s both install %r with different contents or modes"
+                                 % (wheels[old.src - first_src], path, dest))
+            home.setdefault(dest, f)
+    dirs = {posixpath.dirname(d) for d in home}
+    for d in list(dirs):
+        while d:
+            d = posixpath.dirname(d)
+            dirs.add(d)
+    for d in dirs:
+        if d in home:
+            raise ValueError("%s: installed both as a file and as a directory" % d)
+    return home, generated
+
+
+def install(nodes, home, prefix=""):
+    """Move the temporary home's items into the merged tree as pip's _handle_target_dir does without --upgrade: the
+    top-level items of lib/python, then the home's other top-level items (lib excepted), an item whose name the target
+    tree/prefix already holds skipped whole.  Returns the skipped item names."""
+    dirs = set()
+    for p in home:
+        while p:
+            p = posixpath.dirname(p)
+            dirs.add(p)
+    base = prefix[:-1]
+    children = {}
+    for p in list(home) + [d for d in dirs if d]:
+        children.setdefault(posixpath.dirname(p), []).append(p)
+    skipped = []
+    for src_dir, skip in ((_LIB, lambda item: False), ("", lambda item: _LIB.startswith(item))):
+        for item in sorted(posixpath.basename(p) for p in children.get(src_dir, [])):
+            if skip(item):
+                continue
+            target = base + "/" + item if base else item
+            if target in nodes:
+                if lookup(nodes, target) is None:
+                    raise ValueError("%r: the tree holds it as a dangling or looping symlink, which pip would replace"
+                                     % target)
+                skipped.append(item)
+                continue
+            origin = posixpath.join(src_dir, item) if src_dir else item
+            todo = [origin]
+            while todo:
+                p = todo.pop()
+                nodes[target + p[len(origin):]] = home.get(p) or _Dir()
+                todo += children.get(p, [])
+    return skipped
+
+
+def clean(nodes, prefix="", keep_tests=()):
+    """The build script's clean-up lines on tree/prefix, in the model: `*.egg-info` and `*.dist-info` at its top level
+    (shell globs: no dot files), `__pycache__` at any depth, and `tests` at any depth unless the keep pattern
+    (project_build._keep_pattern) matches the path `find ./build/ -name tests` prints, decided by the same regcomp rule
+    as lb2_tree_cleanup.  Removes every node below a match; returns the matches per rule (a match below another
+    counted once, with the outer one)."""
+    from .project_build import _keep_pattern
+    base = prefix[:-1]
+    rel = {p: (p[len(base) + 1:] if base else p) for p in nodes if p and (not base or p.startswith(base + "/"))}
+    hits, tests = {}, []
+    for p, r in rel.items():
+        leaf = posixpath.basename(r)
+        if "/" not in r and not r.startswith(".") and r.endswith((".egg-info", ".dist-info")):
+            hits[p] = r.rsplit(".", 1)[1]
+        elif leaf == "__pycache__":
+            hits[p] = "__pycache__"
+        elif leaf == "tests":
+            tests.append(p)
+    if tests:
+        lib = N.load()
+        lines = (C.c_char_p * len(tests))(*[os.fsencode(BUILD_DIR + rel[p]) for p in tests])
+        out = (C.c_uint8 * len(tests))()
+        rc = lib.lb2_cleanup_tests_removed(os.fsencode(_keep_pattern(keep_tests)), lines, len(tests), out)
+        if rc != N.LB2_OK:
+            raise ValueError("keep_tests %r: not a valid grep pattern" % (list(keep_tests),))
+        hits.update((p, "tests") for p, r in zip(tests, out) if r)
+    counts = {"egg-info": 0, "dist-info": 0, "__pycache__": 0, "tests": 0, "entries": 0}
+
+    def under(p):
+        while p != base and p:
+            p = posixpath.dirname(p)
+            if p in hits:
+                return True
+        return False
+    for p in [p for p in rel if p in hits or under(p)]:
+        if p in hits and not under(p):
+            counts[hits[p]] += 1
+        counts["entries"] += 1
+        del nodes[p]
+    return counts
+
+
+def _entry_info(path, node, size, umask):
+    if not isinstance(node, _WheelFile):
+        return zip_info(path, node, size, umask)
+    zi = zipfile.ZipInfo(path, node.date_time)
+    zi.external_attr = (stat.S_IFREG | node.mode) << 16
+    zi.file_size = size
+    return zi
+
+
+def build_with(dst, tarballs, wheels, reader, indexer, decoder, stripper, encoder, prefix="", keep_tests=(),
+               executable=sys.executable, fallback_host_strip=True, tolerate_non_elf=False):
+    """zip_build with the engines given (tarball.GpuTarReader, tarball.GpuTarIndex, zipfile_gpu.GpuUnzipDecoder,
+    zipfile_gpu.GpuStripper, zipfile_gpu.GpuZipEncoder fed by submit_device, or stand-ins with the same interfaces)."""
+    tarballs, wheels = [os.fspath(t) for t in tarballs], [os.fspath(w) for w in wheels]
+    dst = os.fspath(dst)
+    check_prefix(prefix)
+    if not tarballs and not wheels:
+        raise ValueError("zip_build: no tarball and no wheel")
+    for s in tarballs + wheels:
+        if os.path.realpath(s) == os.path.realpath(dst) or (os.path.exists(dst) and os.path.samefile(s, dst)):
+            raise ValueError("zip_build: %r is a source being read; write the result somewhere else" % dst)
+    if encoder.piece_bytes < Z.CHUNK:
+        raise ValueError("pieces of %d bytes: at least %d are needed" % (encoder.piece_bytes, Z.CHUNK))
+    umask = Z._umask()
+    home, generated = read_home(wheels, umask, executable, len(tarballs))      # a wheel's refusal comes first
+    refs = reader.read_many(tarballs) if tarballs else []
+    listings, views = [], []
+    index = {"kernel_ms": 0.0, "n_members": 0, "ranges": 0, "bytes": 0, "misses": 0, "miss_bytes": 0}
+    for ref in refs:
+        members, _, view, (ranges, data, ist) = T.list_members(ref, indexer, reader)
+        listings.append(members)
+        views.append(view)
+        index["kernel_ms"] += ist.get("kernel_ms", 0.0)
+        index["n_members"] += ist.get("n_members", len(members))
+        index["ranges"] += len(ranges)
+        index["bytes"] += len(data)
+    nodes = merge(listings, prefix)
+    skipped_items = install(nodes, home, prefix)
+    removed = clean(nodes, prefix, keep_tests)
+    entries, skipped_entries = walk(nodes)
+    chosen, skipped = select(nodes)
+    chosen_ids = {id(f) for f in chosen}
+
+    c = {"gpu": 0, "fallback": 0, "skipped": skipped, "in_bytes": 0, "out_bytes": 0, "uploaded": 0}
+    dev, host = {}, {}          # id(node) -> its bytes for the zip: a device ref / bytes to upload after the strip
+
+    def host_fix(data, name):
+        fixed = stripper.host_strip(data) if fallback_host_strip else None
+        if fixed is None:
+            if tolerate_non_elf and data[:4] != b"\x7fELF":
+                c["skipped"] += 1
+                return data
+            raise Z.StripFailed(name, "strip refuses this file (the reference's xargs exits 123)"
+                                if fallback_host_strip else "not stripped on the GPU, and the host strip is off")
+        c["fallback"] += 1
+        c["in_bytes"] += len(data)
+        c["out_bytes"] += len(fixed)
+        return fixed
+
+    def strip(pairs, keep_on_device):
+        """strip [(node, device ref)] in one batch; the results go to dev, or to host when the refs die next"""
+        res = stripper.strip([r for _, r in pairs]) if pairs else []
+        for (f, r), (status, new) in zip(pairs, res):
+            if status == N.ST_OK:
+                c["gpu"] += 1
+                c["in_bytes"] += r[1]
+                c["out_bytes"] += new[1]
+                if keep_on_device:
+                    dev[id(f)] = new
+                else:
+                    host[id(f)] = stripper.fetch(new)
+            elif status == N.ST_NOT_ELF and tolerate_non_elf:
+                c["skipped"] += 1
+                if keep_on_device:
+                    dev[id(f)] = r
+                else:
+                    host[id(f)] = stripper.fetch(r)
+            else:
+                host[id(f)] = host_fix(stripper.fetch(r), f.label())
+
+    # the wheel members decoded on the device: the selected ones, and stored ones (their bodies are no DEFLATE)
+    files = {id(t): t for _, t in entries if isinstance(t, _File)}
+    files.update((id(f), f) for f in chosen)
+    todo = sorted((f for f in files.values() if isinstance(f, _WheelFile) and f.data is None and
+                   (id(f) in chosen_ids or f.member.compress_type != zipfile.ZIP_DEFLATED)),
+                  key=lambda f: f.position())
+    handles = [open(w, "rb") for w in wheels]
+    zfs = [zipfile.ZipFile(h) for h in handles]
+    try:
+        sources = []
+        for zf, h in zip(zfs, handles):
+            h.seek(0, os.SEEK_END)
+            sources.append((zf, h, h.tell()))
+        tar_chosen = [(f, (refs[f.src][0] + f.member.offset_data, f.member.size)) for f in chosen
+                      if not isinstance(f, _WheelFile)]
+        by_id, tar_done = {id(f): f for f in todo}, []
+
+        def decoded(part, got, whole):
+            for key, zi, _ in part:
+                status = got.get(key, (Z.UNZIP_OK, None))[0]
+                if status != Z.UNZIP_OK:
+                    raise Z.BadZipMember(zi.filename, {Z.UNZIP_BAD_DATA: "Invalid DEFLATE data", Z.UNZIP_BAD_CRC:
+                                                       "Bad CRC-32", Z.UNZIP_WRONG_SIZE: "Wrong uncompressed size"}[status])
+            pairs = []
+            for key, zi, (zf, _, _) in part:
+                f = by_id[key]
+                if key not in got:                            # not on the device: read by the stdlib
+                    data = zf.read(zi)
+                    host[key] = host_fix(data, zi.filename) if key in chosen_ids else data
+                elif key in chosen_ids:
+                    pairs.append((f, got[key][1]))
+                elif whole:
+                    dev[key] = got[key][1]
+                else:
+                    host[key] = stripper.fetch(got[key][1])
+            if whole:                                         # every selected file in one strip batch
+                strip(tar_chosen + pairs, True)
+                tar_done.append(True)
+            else:
+                strip(pairs, False)
+        batch = [(id(f), f.member, sources[f.src - len(tarballs)]) for f in todo]
+        if batch:
+            c["uploaded"] += Z.decode_members(decoder, batch, decoded)
+        if not tar_done:                                      # no wheel member, or the wheels' batch was split
+            strip(tar_chosen, True)
+        for f in chosen:                                      # a script made on the host, named *.so
+            if isinstance(f, _WheelFile) and f.data is not None:
+                host[id(f)] = host_fix(f.data, f.label())
+        for f in files.values():
+            if isinstance(f, _WheelFile) and f.data is not None and id(f) not in host:
+                host[id(f)] = f.data
+        if host:                                              # one upload for every file made on the host
+            buf, at = bytearray(), {}
+            for k, data in host.items():
+                buf += bytes(-len(buf) % Z.ALIGN)
+                at[k] = (len(buf), len(data))
+                buf += data
+            addr = reader.upload(bytes(buf))
+            for k, (off, n) in at.items():
+                dev[k] = (addr + off, n)
+
+        items, infos, copied = [], [], {}
+        for i, (p, node) in enumerate(entries):
+            ref = None
+            if isinstance(node, _File):
+                ref = dev.get(id(node))
+                if ref is None and not isinstance(node, _WheelFile):
+                    ref = (refs[node.src][0] + node.member.offset_data, node.member.size)
+            if ref is not None:
+                items.append((i, ref))
+                infos.append((None, _entry_info(p, node, ref[1], umask)))
+            elif isinstance(node, _WheelFile):                # a DEFLATE body copied from its wheel
+                zi = _entry_info(p, node, node.member.file_size, umask)
+                zi.compress_type, zi.CRC, zi.compress_size = zipfile.ZIP_DEFLATED, node.member.CRC, node.member.compress_size
+                copied[i] = node
+                infos.append((None, zi))
+            else:
+                infos.append((None, _entry_info(p, node, 0, umask)))
+
+        out_dir = os.path.dirname(dst) or "."
+        os.makedirs(out_dir, exist_ok=True)
+        fd, tmp = tempfile.mkstemp(prefix=os.path.basename(dst) + ".", suffix=".tmp", dir=out_dir)
+        downloaded = 0
+        try:
+            with os.fdopen(fd, "w+b") as fp:
+                position = {id(zi): i for i, (_, zi) in enumerate(infos)}
+
+                def copy(zi):
+                    node = copied.get(position[id(zi)])
+                    if node is None:                          # a directory
+                        zi.compress_size = zi.CRC = 0
+                        fp.write(zi.FileHeader(False))
+                        return
+                    zf, h, _ = sources[node.src - len(tarballs)]
+                    start = _body_offset(h, node.member)
+                    fp.write(zi.FileHeader())
+                    h.seek(start)
+                    left = node.member.compress_size
+                    while left:
+                        block = h.read(min(left, 1 << 20))
+                        if not block:
+                            raise zipfile.BadZipFile("%s ends inside the body of %r" % (zf.filename, node.member.filename))
+                        fp.write(block)
+                        left -= len(block)
+
+                w = Z._ContainerWriter(fp, infos, copy=copy)
+                for i, node in copied.items():                # a body copied as it is keeps its seek table
+                    field = ST.zip_field_of(node.member.extra)
+                    if field:
+                        w.tables[i] = field
+                in_flight = []
+
+                def collect():
+                    nonlocal downloaded
+                    body, res = encoder.collect()
+                    downloaded += len(body)
+                    chunks = getattr(encoder, "seek_chunks", None) or [None] * len(res)
+                    for (idx, (_, nbytes)), (off, k, crc, ended), ch in zip(in_flight.pop(0), res, chunks):
+                        w.part(idx, body[off:off + k], crc, ended, nbytes, ch)
+
+                for segs, flags in Z._device_pieces(items, encoder.piece_bytes, encoder.max_segs):
+                    encoder.submit_device([ref for _, ref in segs], flags)
+                    in_flight.append(segs)
+                    if len(in_flight) == 2:
+                        collect()
+                while in_flight:
+                    collect()
+                w.finish()
+                zip_bytes = fp.tell()
+            os.chmod(tmp, 0o666 & ~umask)
+            os.replace(tmp, dst)
+        except BaseException:
+            os.unlink(tmp)
+            raise
+    finally:
+        for zf in zfs:
+            zf.close()
+        for h in handles:
+            h.close()
+    index["misses"] = sum(v.misses for v in views)
+    index["miss_bytes"] = sum(v.miss_bytes for v in views)
+    n_copied = len(copied)
+    st = {"sources": len(tarballs), "wheels": len(wheels), "members": sum(len(m) for m in listings),
+          "wheel_members": sum(1 for z in zfs for zi in z.infolist() if not zi.is_dir()),
+          "entries": len(infos), "files": w.n_files + n_copied, "skipped_entries": skipped_entries,
+          "selected": len(chosen), "gpu": c["gpu"], "fallback": c["fallback"], "skipped": c["skipped"],
+          "in_bytes": c["in_bytes"], "out_bytes": c["out_bytes"],
+          "copied": {"members": n_copied, "bytes": sum(n.member.compress_size for n in copied.values()),
+                     "file_bytes": sum(n.member.file_size for n in copied.values())},
+          "generated_scripts": generated, "removed": removed, "skipped_items": skipped_items,
+          "file_bytes": w.in_bytes, "deflated_bytes": w.out_bytes, "tar_bytes_in": sum(n for _, n in refs),
+          "src_bytes": sum(os.path.getsize(s) for s in tarballs + wheels), "zip_bytes": zip_bytes,
+          "uploaded_bytes": reader.uploaded + c["uploaded"] + stripper.uploaded,
+          "downloaded_bytes": reader.downloaded + 16 * index["ranges"] + index["bytes"] + downloaded +
+          stripper.downloaded,
+          "index": index, "inflate": reader.stats() if tarballs else {}, "unzip": decoder.stats(),
+          "strip": stripper.stats(), "deflate": encoder.stats()}
+    st["kernel_ms"] = (st["inflate"].get("kernel_ms", 0.0) + index["kernel_ms"] + st["unzip"].get("kernel_ms", 0.0) +
+                       sum(st["strip"].values()) + st["deflate"].get("kernel_ms", 0.0))
+    return st
+
+
+def _body_offset(f, zi):
+    """the offset of zi's body in the open archive f, from its local header"""
+    f.seek(zi.header_offset)
+    fh = f.read(zipfile.sizeFileHeader)
+    if len(fh) != zipfile.sizeFileHeader or fh[:4] != zipfile.stringFileHeader:
+        raise zipfile.BadZipFile("Bad magic number for file header of %r" % zi.filename)
+    fh = struct.unpack(zipfile.structFileHeader, fh)
+    return zi.header_offset + zipfile.sizeFileHeader + fh[zipfile._FH_FILENAME_LENGTH] + fh[zipfile._FH_EXTRA_FIELD_LENGTH]
+
+
+def zip_build(dst, tarballs=(), wheels=(), prefix="", keep_tests=(), executable=sys.executable, ctx=None,
+              compresslevel=None, fallback_host_strip=True, tolerate_non_elf=False, piece_bytes=PIECE_BYTES,
+              seek_table=False):
+    """Write the Lambda zip `dst` of a whole build -- prebuilt package tarballs and wheels -- as `lambdipy build`
+    leaves it, without unpacking anything: entry for entry the zip these passes give, with T = tree / prefix:
+    `tarfile.open(t, "r:gz").extractall(T, filter="fully_trusted")` for each tarball in order, `pip install --no-deps
+    --no-index --target T W1.whl W2.whl ...` (pip 24, no --upgrade), the build script's clean-up lines on T (`rm -rf
+    *.egg-info *.dist-info`, `find -name __pycache__ | xargs rm -rf`, `find -name tests | grep -v PATTERN | xargs rm
+    -rf` with PATTERN project_build._keep_pattern(keep_tests)), `find T -name "*.so" | xargs strip`, and
+    `shutil.make_archive` of tree, the entries in the order of os.walk listing every directory sorted.
+
+    pip is restated on a model of the tree, not run (read_wheel, read_home, install): root members and
+    <name>.data/{purelib,platlib} go to lib/python of a temporary home, scripts to bin, headers to
+    include/site/pythonX.Y/<name>, data to the home itself; a `.data/scripts` file starting `#!python` gets
+    `#!<executable>` (pip's fix_script); console and gui entry points become scripts in bin with pip 24's launcher
+    text.  A member with an executable bit gets mode 0o777 & ~umask | 0o111, any other file 0o666 & ~umask (a fixed
+    script keeps its member's rule), a generated script 0o666 & ~umask | 0o555 (distlib's set_mode).  The home's
+    lib/python items, then its other top-level items (lib excepted), move into T; an item T already holds (from a
+    tarball) is skipped whole, as pip warns and skips without --upgrade (stats skipped_items).  Two wheels may install
+    the same path only with the same size, CRC-32 and mode (the entry keeps the first wheel's date); any other
+    overlap, a distribution given twice, a wheel without exactly one .dist-info or with a Wheel-Version other than
+    1.x, a member leaving the tree, an encrypted member or one compressed with anything but stored or deflated, and
+    the tarball merges zip_tarballs refuses raise ValueError before dst exists.  Compatibility tags are not checked:
+    the wheels are the ones downloaded for Lambda's platform.  The clean-up covers the tarballs' files too.
+
+    Data path: a wheel file that is not stripped keeps its DEFLATE body, copied from the wheel with the CRC-32 and
+    sizes of its central directory (its CRC is not checked, as in zipfile_gpu.strip_zip); it never crosses the bus.
+    The `*.so` files select chooses in the final tree are stripped on the GPU: the wheel members among them (and any
+    stored member) are uploaded in one buffer and inflated in one decoder run (zipfile_gpu.decode_members, split in
+    halves when the device is too small), then stripped in one batch with the tarballs' files, with the host-strip
+    fallback.  Scripts made on the host are uploaded once.  Every rewritten body is deflated on the GPU; compresslevel
+    and seek_table apply to those bodies.
+
+    Deviations, where the passes would record the time they ran: zip_tarballs' list, and a wheel file keeps its
+    member's date_time, a generated script takes the date_time of its wheel's entry_points.txt, a directory pip makes
+    gets 1980-01-01 00:00:00 and 0o777 & ~umask, and a directory that loses children to the clean-up keeps its own
+    date.  Entry points named pip or easy_install (which pip installs under several names) raise ValueError.
+
+    Returns zip_tarballs' stats dict with wheels, wheel_members, copied (members, bytes, file_bytes),
+    generated_scripts, removed (the clean-up's matches per rule and the entries removed), skipped_items and unzip (the
+    decoder's stats) added.  There is no CPU path: without a GPU this raises."""
+    N.deflate_flags(compresslevel)
+    check_prefix(prefix)
+    own = False
+    if ctx is None:
+        ctx, own = T._default_context()
+    try:
+        with T.GpuTarReader(ctx) as reader, Z.GpuUnzipDecoder(ctx) as dec, Z.GpuStripper(ctx) as stripper, \
+                Z.GpuZipEncoder(ctx, piece_bytes, compresslevel=compresslevel, host_buffers=False,
+                                seek_table=seek_table) as enc:
+            return build_with(dst, tarballs, wheels, reader, T.GpuTarIndex(ctx), dec, stripper, enc, prefix,
+                              keep_tests, executable, fallback_host_strip, tolerate_non_elf)
+    finally:
+        if own:
+            ctx.close()
+
+
 def main(argv=None):
-    """python -m lambdipy_b200.layer DST SRC [SRC ...] [--prefix python/] [--level 9] [--seek-table]"""
+    """python -m lambdipy_b200.layer DST [SRC ...] [--wheel WHL ...] [--keep-tests NAME ...] [--clean]
+    [--prefix python/] [--level 9] [--seek-table]"""
     import argparse
     ap = argparse.ArgumentParser(prog="python -m lambdipy_b200.layer",
                                  description="write the Lambda zip of .tar.gz package assets, shared objects stripped, "
                                              "inflated, stripped and deflated on the GPU")
     ap.add_argument("dst")
-    ap.add_argument("srcs", nargs="+", metavar="src")
+    ap.add_argument("srcs", nargs="*", metavar="src")
+    ap.add_argument("--wheel", action="append", default=[], metavar="WHL",
+                    help="install this wheel as `pip install --no-deps --target` would (repeatable; implies --clean)")
+    ap.add_argument("--keep-tests", action="append", default=[], metavar="NAME",
+                    help="keep the tests directories whose path contains NAME (repeatable)")
+    ap.add_argument("--clean", action="store_true",
+                    help="run the build script's clean-up lines (*.egg-info, *.dist-info, __pycache__, tests)")
     ap.add_argument("--prefix", default="", help='directory of the zip the sources go under ("python/" for a layer)')
     ap.add_argument("--level", type=int, choices=[9], default=None, help="9: the optimal parse (smaller, slower)")
     ap.add_argument("--seek-table", action="store_true",
                     help="give multi-chunk members seek tables, with which the GPU reader decodes them without search")
     args = ap.parse_args(argv)
+    if not args.srcs and not args.wheel:
+        ap.error("give at least one tarball or --wheel")
+    if args.wheel or args.clean:
+        st = zip_build(args.dst, args.srcs, args.wheel, prefix=args.prefix, keep_tests=args.keep_tests,
+                       compresslevel=args.level, **ST.seek_kw(args.seek_table))
+        print("Layer zip: %s, %.1f MB from %d tarballs and %d wheels (%.1f MB), %d entries; %d bodies copied, %d "
+              "entries cleaned up; %d shared objects stripped (%d via host strip), %.1f MB -> %.1f MB"
+              % (args.dst, st["zip_bytes"] / 1e6, len(args.srcs), len(args.wheel), st["src_bytes"] / 1e6,
+                 st["entries"], st["copied"]["members"], st["removed"]["entries"], st["gpu"] + st["fallback"],
+                 st["fallback"], st["in_bytes"] / 1e6, st["out_bytes"] / 1e6))
+        return 0
+    if args.keep_tests:
+        ap.error("--keep-tests needs --clean or --wheel")
     st = zip_tarballs(args.srcs, args.dst, prefix=args.prefix, compresslevel=args.level, **ST.seek_kw(args.seek_table))
     print("Layer zip: %s, %.1f MB from %d tarballs (%.1f MB), %d entries; %d shared objects stripped (%d via host "
           "strip), %.1f MB -> %.1f MB"

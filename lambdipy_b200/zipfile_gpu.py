@@ -763,8 +763,8 @@ def host_strip(data):
 class GpuStripper:
     """lb2_strip_device_async / lb2_batch_results over files that already lie in device memory.
 
-    strip(refs): refs are (address, size) with every address a multiple of 16 inside one device buffer (the
-    decoder's); returns [(LB2_ST_* status, (address, size) of the stripped file in the output arena)], valid until
+    strip(refs): refs are (address, size) with every address a multiple of 16 (each file is read at its own address,
+    so they may lie in several device buffers, such as a tar arena and the decoder's output); returns [(LB2_ST_* status, (address, size) of the stripped file in the output arena)], valid until
     the next strip().  fetch(ref) brings a file to the host and upload(data) puts one on the device (until the next
     strip()): the two directions of the host-strip fallback, counted in uploaded / downloaded.  host_strip is the
     fallback itself."""
@@ -883,6 +883,49 @@ def _device_pieces(items, piece, max_segs):
         yield segs, N.ZIP_CONTINUES if cont else 0
 
 
+def decode_members(decoder, batch, consume, _whole=True):
+    """Inflate the members of a batch [(key, ZipInfo, (ZipFile, its open file, its size))] on the device: every body is
+    read into one upload buffer and the decoder's run_device takes them all, reading a member's seek table when it has
+    one.  When the batch does not fit on the device (DeviceTooSmall) it is split in halves, each decoded on its own.
+    consume(part, decoded, whole) is called once per part that was decoded, in order: part is a slice of the batch,
+    decoded {key: (UNZIP_* status, (device address, size))} holds the members the decoder took, valid until the
+    decoder's next run (the next part's, when the batch was split), and whole says whether part is the entire batch.
+    A member the GPU reader does not take (another method, encryption, a local header the stdlib refuses) or that
+    does not fit on the device alone has no entry: the stdlib's own code reads it.  Returns the body bytes uploaded."""
+    view = decoder.buffer(sum(zi.compress_size for _, zi, _ in batch))
+    members, taken, tables, fill = [], [], [], 0
+    for key, zi, (zf, src, archive_bytes) in batch:
+        if not _gpu_member(zi):
+            continue
+        src.seek(zi.header_offset)
+        head = src.read(zipfile.sizeFileHeader)
+        if len(head) == zipfile.sizeFileHeader:
+            fh = struct.unpack(zipfile.structFileHeader, head)
+            head += src.read(fh[zipfile._FH_FILENAME_LENGTH] + fh[zipfile._FH_EXTRA_FIELD_LENGTH])
+        b = _body(zf, zi, head, zi.header_offset, archive_bytes)
+        if b is None or b[0] != len(head):
+            continue                       # the stdlib's own code reads it, and raises what it raises
+        if b[1] < 0 or _read_into(src, view[fill:fill + zi.compress_size]) != zi.compress_size:
+            raise BadZipMember(zi.filename, "The archive ends inside the body")
+        members.append((fill, zi.compress_size, zi.file_size, zi.CRC, zi.compress_type))
+        taken.append(key)
+        tables.append(_seek_entries(zi))
+        fill += zi.compress_size
+    decoded, uploaded = {}, 0
+    try:
+        if taken:
+            res = decoder.run_device(fill, members, tables=tables) if any(tables) else decoder.run_device(fill, members)
+            decoded, uploaded = dict(zip(taken, res)), fill
+    except DeviceTooSmall:
+        if len(taken) > 1:
+            half = len(batch) // 2
+            return decode_members(decoder, batch[:half], consume, False) + \
+                decode_members(decoder, batch[half:], consume, False)
+        # a member that does not fit on the device alone: read by the stdlib
+    consume(batch, decoded, _whole)
+    return uploaded
+
+
 def strip_with(src_zip, dst_zip, decoder, stripper, encoder, fallback_host_strip=True, tolerate_non_elf=False,
                batch_bytes=BATCH_BYTES):
     """strip_zip with the three engines given (GpuUnzipDecoder, GpuStripper, GpuZipEncoder, or stand-ins with the
@@ -930,6 +973,7 @@ def strip_with(src_zip, dst_zip, decoder, stripper, encoder, fallback_host_strip
                     left -= len(block)
 
             w = _ContainerWriter(fp, entries, copy=copy_member)
+            source = (zf, src, archive_bytes)
             for idx, zi in enumerate(zf.filelist):   # a member copied as it is keeps its seek table
                 field = ST.zip_field_of(zi.extra)
                 if field:
@@ -957,38 +1001,10 @@ def strip_with(src_zip, dst_zip, decoder, stripper, encoder, fallback_host_strip
 
             def run(batch):
                 """batch: [(entry index, source ZipInfo)] of selected members, in archive order"""
-                view = decoder.buffer(sum(zi.compress_size for _, zi in batch))
-                members, taken, tables, fill = [], [], [], 0
-                for idx, zi in batch:
-                    if not _gpu_member(zi):
-                        continue
-                    src.seek(zi.header_offset)
-                    head = src.read(zipfile.sizeFileHeader)
-                    if len(head) == zipfile.sizeFileHeader:
-                        fh = struct.unpack(zipfile.structFileHeader, head)
-                        head += src.read(fh[zipfile._FH_FILENAME_LENGTH] + fh[zipfile._FH_EXTRA_FIELD_LENGTH])
-                    b = _body(zf, zi, head, zi.header_offset, archive_bytes)
-                    if b is None or b[0] != len(head):
-                        continue                       # the stdlib's own code reads it, and raises what it raises
-                    if b[1] < 0 or _read_into(src, view[fill:fill + zi.compress_size]) != zi.compress_size:
-                        raise BadZipMember(zi.filename, "The archive ends inside the body")
-                    members.append((fill, zi.compress_size, zi.file_size, zi.CRC, zi.compress_type))
-                    taken.append(idx)
-                    tables.append(_seek_entries(zi))
-                    fill += zi.compress_size
-                decoded = {}
-                try:
-                    if taken:
-                        res = decoder.run_device(fill, members, tables=tables) if any(tables) else \
-                            decoder.run_device(fill, members)
-                        decoded = dict(zip(taken, res))
-                        n["uploaded"] += fill
-                except DeviceTooSmall:
-                    if len(taken) > 1:
-                        run(batch[:len(batch) // 2])
-                        run(batch[len(batch) // 2:])
-                        return
-                    # a member that does not fit on the device alone: read by the stdlib, stripped on the host
+                n["uploaded"] += decode_members(decoder, [(idx, zi, source) for idx, zi in batch], finish)
+
+            def finish(part, decoded, whole):
+                batch = [(idx, zi) for idx, zi, _ in part]
                 for idx, zi in batch:
                     status = decoded.get(idx, (UNZIP_OK, None))[0]
                     if status != UNZIP_OK:
