@@ -487,6 +487,57 @@ typedef struct lb2_tar_index_stats {
 int lb2_tar_index(lb2_ctx *ctx, const void *d_tar, uint64_t n, lb2_tar_range *ranges, uint32_t max_ranges,
                   uint32_t *n_ranges, void *h_bytes, uint64_t bytes_cap, uint64_t *n_bytes, lb2_tar_index_stats *stats);
 
+/* ---- dynamic sections: what the loader reads of shared objects in device memory ------------------------------ */
+/* What `readelf -dW` and `readelf -VW` print of each shared object's dependencies -- DT_SONAME, DT_NEEDED, DT_RPATH,
+ * DT_RUNPATH, the version needs and the version definitions -- read where the objects lie, which is how
+ * deps.check_zip tells whether the shared objects of a Lambda zip will load (where the host would inflate every
+ * object, or bring it back over PCIe, and run readelf on it).  Object i is sizes[i] bytes at the device address
+ * d_ptrs[i] (both arrays in host memory; any alignment), such as the (address, size) pairs lb2_unzip_device_output
+ * hands out.  One warp parses each object (kernels in elf_deps.cu, logic in elf_deps.cuh): the ELF header, the
+ * program headers, the dynamic array up to DT_NULL or PT_DYNAMIC's end, and the DT_VERNEED / DT_VERDEF chains, with
+ * addresses mapped through the PT_LOADs.  No byte outside an object's [0, size) is read.
+ *
+ * objects[i] receives the status, e_machine / e_type and where its records and strings are: records[first_record ..
+ * first_record + n_records), in this order -- the string tags in dynamic-array order (DT_NEEDED in the loader's
+ * order), then each Verneed as a VERNEED_FILE record followed by its VERNEED_VERSION records, then the first name of
+ * each Verdef as a VERDEF record -- and their strings, each followed by a NUL, in h_pool[pool_off .. pool_off +
+ * pool_len).  Only LB2_ELF_OK objects have records.  LB2_E_CAPACITY when max_records or pool_cap is too small:
+ * objects[] and stats are filled and *n_records / *pool_bytes say what is needed.  stats.kernel_ms times the two
+ * passes (count, then write at the host's exclusive scan of the counts) with CUDA events. */
+#define LB2_ELF_OK 0
+#define LB2_ELF_NOT_ELF 1            /* no ELF magic                                                                  */
+#define LB2_ELF_UNSUPPORTED 2        /* ELF32 or big-endian: not parsed                                               */
+#define LB2_ELF_STATIC 3             /* no PT_DYNAMIC                                                                 */
+#define LB2_ELF_MALFORMED 4          /* an offset, address or link outside the file or its segment, a string not     */
+                                     /* ended before DT_STRSZ, a chain cut short of its count or past n / 8 entries  */
+#define LB2_ELF_REC_SONAME 1
+#define LB2_ELF_REC_NEEDED 2
+#define LB2_ELF_REC_RPATH 3
+#define LB2_ELF_REC_RUNPATH 4
+#define LB2_ELF_REC_VERNEED_FILE 5     /* vn_file                                                                      */
+#define LB2_ELF_REC_VERNEED_VERSION 6  /* vna_name; flags = vna_flags (2: weak), ref = its VERNEED_FILE record       */
+#define LB2_ELF_REC_VERDEF 7           /* the first vda_name of a Verdef; flags = vd_flags (1: the base version)      */
+typedef struct lb2_elf_object {
+  int32_t status;                 /* LB2_ELF_*                                                                    */
+  uint16_t machine, type;         /* e_machine, e_type (0 unless the header is a complete ELF64 little-endian one) */
+  uint32_t first_record, n_records;
+  uint64_t pool_off, pool_len;
+} lb2_elf_object;
+typedef struct lb2_elf_record {
+  uint32_t kind;                  /* LB2_ELF_REC_*                                                                */
+  uint32_t flags, ref;
+  uint32_t len;                   /* the string's bytes, without its NUL                                          */
+  uint64_t off;                   /* the string in h_pool                                                         */
+} lb2_elf_record;
+typedef struct lb2_elf_deps_stats {
+  uint64_t n_records, pool_bytes; /* needed, also past the capacities                                             */
+  uint64_t bytes_down;            /* device-to-host bytes: the objects, records and pool                          */
+  float kernel_ms;                /* the count and write kernels (CUDA events)                                    */
+} lb2_elf_deps_stats;
+int lb2_elf_deps(lb2_ctx *ctx, const uint64_t *d_ptrs, const uint64_t *sizes, uint32_t n, lb2_elf_object *objects,
+                 lb2_elf_record *records, uint32_t max_records, uint32_t *n_records, void *h_pool, uint64_t pool_cap,
+                 uint64_t *pool_bytes, lb2_elf_deps_stats *stats);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,6 +19,8 @@ Public surface:
                                                 inflated, stripped and deflated on the GPU without unpacking them
     zip_build(dst, tarballs, wheels)            the Lambda zip of a whole build: tarballs and wheels, pip's target
                                                 install and the build script's clean-up restated, strip on the GPU
+    check_zip(zip_path, mount="/var/task")      whether the zip's shared objects will load on Lambda: dynamic
+                                                sections read on the GPU, the loader's search restated
     patch.apply()                               monkey-patch an installed lambdipy in place
 The byte work is done by liblambdipy_b200.so (CUDA, C ABI in include/lambdipy_b200.h).
 """
@@ -38,4 +40,7 @@ def __getattr__(name):
     if name in ("zip_tarballs", "zip_build"):
         from . import layer
         return getattr(layer, name)
+    if name == "check_zip":
+        from . import deps
+        return deps.check_zip
     raise AttributeError(name)

@@ -31,10 +31,13 @@ EXPORTS = [
     "lb2_zip_submit_device", "lb2_unzip_device_output",
     "lb2_inflate_device_output", "lb2_memcpy_d2d", "lb2_gzip_submit_device", "lb2_tar_index",
     "lb2_gzip_chunk_sizes", "lb2_inflate_run_table", "lb2_zip_chunk_sizes", "lb2_unzip_run_table",
-    "lb2_cleanup_tests_removed",
+    "lb2_cleanup_tests_removed", "lb2_elf_deps",
 ]
 TAR_STOP_ZERO, TAR_STOP_BAD_HEADER, TAR_STOP_END, TAR_STOP_UNSUPPORTED = 1, 2, 3, 4
 ZIP_CONTINUES, ZIP_MORE = 1, 2
+ELF_OK, ELF_NOT_ELF, ELF_UNSUPPORTED, ELF_STATIC, ELF_MALFORMED = 0, 1, 2, 3, 4  # LB2_ELF_*
+ELF_REC_SONAME, ELF_REC_NEEDED, ELF_REC_RPATH, ELF_REC_RUNPATH = 1, 2, 3, 4  # LB2_ELF_REC_*
+ELF_REC_VERNEED_FILE, ELF_REC_VERNEED_VERSION, ELF_REC_VERDEF = 5, 6, 7
 DEFLATE_BEST = 1  # LB2_DEFLATE_BEST
 
 
@@ -150,6 +153,24 @@ class TarRange(C.Structure):
 
 class TarIndexStats(C.Structure):
     _fields_ = [("n_members", C.c_uint64), ("stop_offset", C.c_uint64), ("stop_reason", C.c_uint32),
+                ("kernel_ms", C.c_float)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class ElfObject(C.Structure):
+    _fields_ = [("status", C.c_int32), ("machine", C.c_uint16), ("type", C.c_uint16), ("first_record", C.c_uint32),
+                ("n_records", C.c_uint32), ("pool_off", C.c_uint64), ("pool_len", C.c_uint64)]
+
+
+class ElfRecord(C.Structure):
+    _fields_ = [("kind", C.c_uint32), ("flags", C.c_uint32), ("ref", C.c_uint32), ("len", C.c_uint32),
+                ("off", C.c_uint64)]
+
+
+class ElfDepsStats(C.Structure):
+    _fields_ = [("n_records", C.c_uint64), ("pool_bytes", C.c_uint64), ("bytes_down", C.c_uint64),
                 ("kernel_ms", C.c_float)]
 
     def as_dict(self):
@@ -292,6 +313,9 @@ def load():
                                         C.POINTER(InflateSpan), u64p, C.POINTER(UnzipResult), C.POINTER(UnzipStats),
                                         u32p, u32p]
     lib.lb2_unzip_run_table.restype = C.c_int
+    lib.lb2_elf_deps.argtypes = [vp, u64p, u64p, C.c_uint32, C.POINTER(ElfObject), C.POINTER(ElfRecord), C.c_uint32,
+                                 u32p, vp, C.c_uint64, u64p, C.POINTER(ElfDepsStats)]
+    lib.lb2_elf_deps.restype = C.c_int
     _lib = lib
     return lib
 

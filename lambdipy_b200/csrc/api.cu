@@ -1653,3 +1653,83 @@ int lb2_tar_index(lb2_ctx *ctx, const void *d_tar, uint64_t n, lb2_tar_range *ra
 }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------------------- dynamic sections
+// The count and write kernels (elf_deps.cu) on the context's stream, the exclusive scan of the counts on the host in
+// between; everything lives in one scratch allocation of the call.
+#include "elf_deps.cuh"
+static_assert(sizeof(lb2_elf_object) == sizeof(elfd::Object), "the count kernel writes lb2_elf_object records");
+static_assert(sizeof(lb2_elf_record) == sizeof(elfd::Record), "the write kernel writes lb2_elf_record records");
+
+extern "C" {
+
+int lb2_elf_deps(lb2_ctx *ctx, const uint64_t *d_ptrs, const uint64_t *sizes, uint32_t n, lb2_elf_object *objects,
+                 lb2_elf_record *records, uint32_t max_records, uint32_t *n_records, void *h_pool, uint64_t pool_cap,
+                 uint64_t *pool_bytes, lb2_elf_deps_stats *stats) {
+  if (!ctx) return LB2_E_ARG;
+  if ((n && (!d_ptrs || !sizes || !objects)) || !n_records || !pool_bytes || (!records && max_records) || (!h_pool && pool_cap)) {
+    ctx->err = "NULL argument";
+    return LB2_E_ARG;
+  }
+  for (uint32_t i = 0; i < n; i++)
+    if (!d_ptrs[i] && sizes[i]) { ctx->err = "lb2_elf_deps: a NULL object address"; return LB2_E_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  const uint64_t job_bytes = 2 * sizeof(uint64_t) * (uint64_t)n, obj_bytes = sizeof(lb2_elf_object) * (uint64_t)n;
+  const uint64_t rec_bytes = sizeof(lb2_elf_record) * (uint64_t)max_records, head = job_bytes + obj_bytes;
+  uint8_t *d_ws = nullptr;
+  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+  float ms[2] = {0, 0};
+  uint64_t total_rec = 0, total_pool = 0, down = 0;
+  bool fits = true;
+  cudaError_t e = cudaMalloc(&d_ws, head + rec_bytes + pool_cap + 16);
+  for (auto &v : ev)
+    if (e == cudaSuccess) e = cudaEventCreate(&v);
+  const uint64_t *d_p = reinterpret_cast<const uint64_t *>(d_ws), *d_s = d_p + n;
+  void *d_obj = d_ws + job_bytes;
+  if (e == cudaSuccess && n) e = cudaMemcpyAsync(d_ws, d_ptrs, job_bytes / 2, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess && n) e = cudaMemcpyAsync(d_ws + job_bytes / 2, sizes, job_bytes / 2, cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[0], ctx->stream);
+  if (e == cudaSuccess) {
+    launch_elf_deps_count(d_p, d_s, n, d_obj, ctx->stream);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaEventRecord(ev[1], ctx->stream);
+  if (e == cudaSuccess && n) e = cudaMemcpyAsync(objects, d_obj, obj_bytes, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  if (e == cudaSuccess) e = cudaEventElapsedTime(&ms[0], ev[0], ev[1]);
+  if (e == cudaSuccess) {
+    down += obj_bytes;
+    for (uint32_t i = 0; i < n; i++) {  // the exclusive scan
+      objects[i].first_record = (uint32_t)total_rec;
+      objects[i].pool_off = total_pool;
+      total_rec += objects[i].n_records;
+      total_pool += objects[i].pool_len;
+    }
+    fits = total_rec <= max_records && total_pool <= pool_cap;
+    if (total_rec > UINT32_MAX) fits = false;
+  }
+  if (e == cudaSuccess && fits && total_rec) {
+    e = cudaMemcpyAsync(d_obj, objects, obj_bytes, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaEventRecord(ev[2], ctx->stream);
+    if (e == cudaSuccess) {
+      launch_elf_deps_write(d_p, d_s, n, d_obj, d_ws + head, d_ws + head + rec_bytes, pool_cap, ctx->stream);
+      e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaEventRecord(ev[3], ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(records, d_ws + head, total_rec * sizeof(lb2_elf_record), cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess && total_pool) e = cudaMemcpyAsync(h_pool, d_ws + head + rec_bytes, total_pool, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms[1], ev[2], ev[3]);
+    down += total_rec * sizeof(lb2_elf_record) + total_pool;
+  }
+  cudaFree(d_ws);
+  for (auto &v : ev) if (v) cudaEventDestroy(v);
+  if (e != cudaSuccess) { ctx->err = std::string("lb2_elf_deps: ") + cudaGetErrorString(e); return LB2_E_CUDA; }
+  *n_records = total_rec > UINT32_MAX ? UINT32_MAX : (uint32_t)total_rec;
+  *pool_bytes = total_pool;
+  if (stats) *stats = lb2_elf_deps_stats{total_rec, total_pool, down, ms[0] + ms[1]};
+  if (!fits) { ctx->err = "lb2_elf_deps: records or pool exceed the capacity given (*n_records, *pool_bytes needed)"; return LB2_E_CAPACITY; }
+  return LB2_OK;
+}
+
+}  // extern "C"

@@ -1,0 +1,532 @@
+"""Will the shared objects of a Lambda zip load there?  `check_zip(zip_path)` reads the dynamic sections of every
+shared object the zip's `import`s would load, on the GPU where the zip reader leaves the decoded bytes
+(lb2_elf_deps), and restates the dynamic loader's search for each one.
+
+    python -m lambdipy_b200.deps ZIP [--mount DIR] [--arch x86_64|arm64] [--provided NAME]...
+                                     [--max-version GLIBC_2.26]... [--ld-library-path P] [--json]
+
+A layer fails at the first `import` when a shared object cannot load: a DT_NEEDED library that neither the zip nor
+the runtime has, a symbol version newer than the runtime's, an object for the other architecture.  The check finds
+these before the upload instead of in a traceback afterwards.
+
+Roots are the members the strip line selects (a regular file whose basename ends in ".so"); member `a/b.so` lies at
+`mount/a/b.so` (/var/task for a function bundle, /opt for a layer written with prefix="python/").  For each root the
+closure is what `dlopen` of that root would load, restated from glibc's _dl_map_object: breadth first over DT_NEEDED
+in dynamic-array order; a name already matching an object of that closure (the name it was loaded by, or its
+DT_SONAME) is that object; a name with a '/' is a path; otherwise the directories of DT_RPATH of the object and of its
+loader chain (not when the object has DT_RUNPATH, and an object's DT_RPATH counts for nothing when it has DT_RUNPATH),
+then `ld_library_path`, then the object's DT_RUNPATH, then the runtime's own libraries.  $ORIGIN, $LIB and $PLATFORM
+are expanded against the path the object was found at.  Symlink members are followed inside the zip, up to 40 hops.
+
+Members are decoded and parsed in rounds: the roots first, then whatever they reach inside the zip that has not been
+parsed yet, and so on.  The GPU reader decodes each round (halving on a device too small); a member it does not take
+is read by the stdlib and uploaded.
+
+`provided` is the set of sonames the runtime image supplies from its own directories (/lib64, /usr/lib64, and the
+loader's defaults).  The default -- glibc's libraries plus libgcc_s.so.1, libstdc++.so.6 and libz.so.1 -- is a guess
+that nobody has checked against a Lambda image here; the report names every need that the list satisfied
+(`provided_used`), so nothing is hidden behind it.
+
+Deviations from the loader, each documented in DESIGN.md section 9.8: a candidate file is taken when it exists (glibc
+also skips a candidate of the wrong ELF class or machine and searches on; here that is an `arch` problem); the
+executable's own DT_RPATH, ld.so.cache entries beyond `provided`, libraries opened by `dlopen` at run time and the
+effects of import order between roots are not modelled; symbol resolution is checked only as far as version needs."""
+import json
+import os
+import posixpath
+import re
+import stat
+import sys
+import zipfile
+
+import ctypes as C
+
+from . import _native as N
+from . import zipfile_gpu as Z
+
+LAMBDA_LD_LIBRARY_PATH = "/var/lang/lib:/lib64:/usr/lib64:/var/runtime:/var/runtime/lib:/var/task:/var/task/lib:/opt/lib"
+LAMBDA_TASK_ROOT = "/var/task"      # the working directory of a Lambda function: relative names resolve there
+RUNTIME_DIRS = ("/lib64", "/usr/lib64")  # where the runtime image keeps the `provided` libraries
+DEFAULT_PROVIDED = frozenset([
+    "ld-linux-x86-64.so.2", "libc.so.6", "libm.so.6", "libpthread.so.0", "libdl.so.2", "librt.so.1", "libutil.so.1",
+    "libresolv.so.2", "libnsl.so.1", "libanl.so.1", "libmvec.so.1", "libgcc_s.so.1", "libstdc++.so.6", "libz.so.1"])
+MACHINES = {"x86_64": 62, "arm64": 183}
+PLATFORMS = {"x86_64": "x86_64", "arm64": "aarch64"}
+STATUS_NAMES = {N.ELF_OK: "ok", N.ELF_NOT_ELF: "not ELF", N.ELF_UNSUPPORTED: "unsupported", N.ELF_STATIC: "static",
+                N.ELF_MALFORMED: "malformed"}
+SYMLINK_HOPS = 40
+BATCH_BYTES = Z.BATCH_BYTES
+_VERSION = re.compile(r"^([A-Za-z][A-Za-z0-9]*)_(\d+(?:\.\d+)*)$")
+VER_FLG_WEAK = 2
+
+
+class GpuElfParser:
+    """lb2_elf_deps over objects in device memory.  parse(refs): refs are (device address, size) pairs; returns
+    [(status, machine, [(kind, flags, ref, name)])].  upload(data) puts a member the GPU reader did not take on the
+    device until the next parse(); uploaded / downloaded count the bytes that crossed the bus."""
+
+    def __init__(self, ctx):
+        self._ctx, self._extra = ctx, []
+        self.uploaded = self.downloaded = 0
+        self._rec_cap, self._pool_cap = 1 << 12, 1 << 18
+        self._stats = {"kernel_ms": 0.0, "objects": 0, "calls": 0}
+
+    def _release(self):
+        for p in self._extra:
+            self._ctx.dev_free(p)
+        self._extra = []
+
+    def parse(self, refs):
+        n = len(refs)
+        if not n:
+            self._release()
+            return []
+        ptrs = (C.c_uint64 * n)(*[a for a, _ in refs])
+        sizes = (C.c_uint64 * n)(*[k for _, k in refs])
+        objs, nr, npool, st = (N.ElfObject * n)(), C.c_uint32(), C.c_uint64(), N.ElfDepsStats()
+        lib, ctx = self._ctx.lib, self._ctx
+        while True:
+            recs = (N.ElfRecord * self._rec_cap)()
+            pool = C.create_string_buffer(self._pool_cap)
+            rc = lib.lb2_elf_deps(ctx.h, ptrs, sizes, n, objs, recs, self._rec_cap, C.byref(nr), pool, self._pool_cap,
+                                  C.byref(npool), C.byref(st))
+            self._stats["kernel_ms"] += st.kernel_ms
+            self.downloaded += st.bytes_down
+            if rc == N.LB2_E_CAPACITY:
+                self._rec_cap = max(self._rec_cap, nr.value)
+                self._pool_cap = max(self._pool_cap, npool.value)
+                continue
+            ctx.check(rc)
+            break
+        self._release()
+        self._stats["objects"] += n
+        self._stats["calls"] += 1
+        return decode(objs, recs, pool.raw[:npool.value])
+
+    def upload(self, data):
+        p = self._ctx.dev_alloc(max(len(data), 1))
+        self._extra.append(p)
+        if data:
+            self._ctx.h2d(p, data, len(data))
+        self.uploaded += len(data)
+        return p, len(data)
+
+    def stats(self):
+        return dict(self._stats)
+
+    def close(self):
+        self._release()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+def decode(objs, recs, pool):
+    """lb2_elf_object / lb2_elf_record arrays and the pool -> [(status, machine, [(kind, flags, ref, name)])]"""
+    out = []
+    for o in objs:
+        rs = []
+        for r in recs[o.first_record:o.first_record + o.n_records]:
+            rs.append((r.kind, r.flags, r.ref, pool[r.off:r.off + r.len].decode("utf-8", "surrogateescape")))
+        out.append((o.status, o.machine, rs))
+    return out
+
+
+class _Obj:
+    """what the loader model needs of one parsed member"""
+
+    def __init__(self, member, status, machine, records):
+        self.member, self.status, self.machine = member, status, machine
+        self.soname = None
+        self.needed, self.rpath, self.runpath, self.verdef, self.verneed = [], None, None, set(), []
+        files = {}
+        for i, (kind, flags, ref, name) in enumerate(records):
+            if kind == N.ELF_REC_NEEDED:
+                self.needed.append(name)
+            elif kind == N.ELF_REC_SONAME:
+                self.soname = name
+            elif kind == N.ELF_REC_RPATH:
+                self.rpath = name if self.rpath is None else self.rpath + ":" + name
+            elif kind == N.ELF_REC_RUNPATH:
+                self.runpath = name if self.runpath is None else self.runpath + ":" + name
+            elif kind == N.ELF_REC_VERNEED_FILE:
+                files[i] = name
+            elif kind == N.ELF_REC_VERNEED_VERSION:
+                self.verneed.append((files.get(ref, ""), name, bool(flags & VER_FLG_WEAK)))
+            elif kind == N.ELF_REC_VERDEF:
+                self.verdef.add(name)
+        if self.runpath is not None:
+            self.rpath = None  # glibc: DT_RPATH is ignored when DT_RUNPATH is present
+
+
+class _Tree:
+    """The zip as the file system under `mount`: {absolute path: ZipInfo of a regular file | link target}, and the
+    directories its paths imply."""
+
+    def __init__(self, zf, mount):
+        self.mount = posixpath.normpath("/" + mount.strip("/")) if mount.strip("/") else "/"
+        self.files, self.links, self.dirs = {}, {}, {self.mount}
+        d = self.mount
+        while d != "/":
+            d = posixpath.dirname(d)
+            self.dirs.add(d)
+        for zi in zf.infolist():  # a repeated name: the last entry, as getinfo and extractall leave it
+            name = zi.filename.rstrip("/")
+            if not name:
+                continue
+            path = posixpath.normpath(posixpath.join(self.mount, name))
+            d = posixpath.dirname(path)
+            while d not in self.dirs:
+                self.dirs.add(d)
+                d = posixpath.dirname(d)
+            self.files.pop(path, None)
+            self.links.pop(path, None)
+            if zi.is_dir():
+                self.dirs.add(path)
+            elif (zi.external_attr >> 16) & 0o170000 == stat.S_IFLNK:
+                self.links[path] = zf.read(zi).decode("utf-8", "surrogateescape")
+            else:
+                self.files[path] = zi
+
+    def lookup(self, path):
+        """the ZipInfo of the regular file `path` ends at, symlinks followed, or None"""
+        parts, i, cur, hops = [x for x in path.split("/") if x], 0, [], SYMLINK_HOPS
+        while i < len(parts):
+            comp = parts[i]
+            if comp == ".":
+                i += 1
+                continue
+            if comp == "..":
+                cur = cur[:-1]
+                i += 1
+                continue
+            p = "/" + "/".join(cur + [comp])
+            if p in self.links:
+                hops -= 1
+                if hops < 0:
+                    return None
+                t = self.links[p]
+                base = [] if t.startswith("/") else cur
+                parts, i, cur = base + [x for x in t.split("/") if x] + parts[i + 1:], 0, []
+                continue
+            last = i + 1 == len(parts) or all(x in ("", ".") for x in parts[i + 1:])
+            if p in self.files:
+                return self.files[p] if last else None
+            if p not in self.dirs:
+                return None
+            cur.append(comp)
+            i += 1
+        return None
+
+
+def _version_key(v):
+    return tuple(int(x) for x in v.split("."))
+
+
+def _expand(dirs, origin, arch):
+    out = []
+    for d in dirs.split(":"):
+        if d == "":
+            d = LAMBDA_TASK_ROOT  # an empty entry is the working directory
+        for token, value in (("ORIGIN", origin), ("LIB", "lib64"), ("PLATFORM", PLATFORMS[arch])):
+            d = d.replace("${%s}" % token, value).replace("$" + token, value)
+        out.append(d)
+    return out
+
+
+class _Model:
+    """the loader's search for each root's closure over the objects parsed so far"""
+
+    def __init__(self, tree, objs, arch, provided, ld_library_path):
+        self.tree, self.objs, self.arch = tree, objs, arch
+        self.provided = frozenset(provided)
+        self.env = _expand(ld_library_path or "", LAMBDA_TASK_ROOT, arch) if ld_library_path else []
+
+    def _find(self, name, obj_path, chain):
+        """(how, path or None, ZipInfo or None) for NEEDED `name` of the object at obj_path loaded through `chain`"""
+        if "/" in name:
+            path = posixpath.join(LAMBDA_TASK_ROOT, name)
+            zi = self.tree.lookup(path)
+            return ("path", path, zi) if zi is not None else ("missing", None, None)
+        obj = self.objs[id(chain[-1][1])]
+        searches = []
+        if obj.runpath is None:
+            for p, zi in reversed(chain):
+                o = self.objs[id(zi)]
+                if o.rpath is not None:
+                    searches.append(("rpath", _expand(o.rpath, posixpath.dirname(p), self.arch)))
+        searches.append(("ld_library_path", self.env))
+        if obj.runpath is not None:
+            searches.append(("runpath", _expand(obj.runpath, posixpath.dirname(obj_path), self.arch)))
+        for how, dirs in searches:
+            for d in dirs:
+                if name in self.provided and posixpath.normpath(d) in RUNTIME_DIRS:
+                    return "provided", None, None
+                path = posixpath.join(d, name)
+                zi = self.tree.lookup(path)
+                if zi is not None:
+                    return how, path, zi
+        return ("provided", None, None) if name in self.provided else ("missing", None, None)
+
+    def closure(self, root_path, root_zi):
+        """(loaded [(path, ZipInfo)] in load order, [(loader path, its ZipInfo, name, how, path)], unparsed ZipInfos
+        reached)"""
+        loaded = [(root_path, root_zi)]
+        names = {id(root_zi): {root_path}}
+        loader = {id(root_zi): None}
+        provided_loaded = set()
+        resolutions, pending = [], []
+        q = 0
+        while q < len(loaded):
+            path, zi = loaded[q]
+            q += 1
+            obj = self.objs.get(id(zi))
+            if obj is None:
+                pending.append(zi)
+                continue
+            if obj.status != N.ELF_OK:
+                continue
+            chain, z = [], zi  # this object, its loader, and on up to the root
+            while z is not None:
+                chain.insert(0, (next(p for p, y in loaded if y is z), z))
+                z = loader[id(z)]
+            for name in obj.needed:
+                hit = next((y for p, y in loaded if name in names[id(y)] or
+                            (id(y) in self.objs and self.objs[id(y)].soname == name)), None)
+                if hit is not None:
+                    resolutions.append((path, zi, name, "loaded", next(p for p, y in loaded if y is hit)))
+                    names[id(hit)].add(name)
+                    continue
+                if name in provided_loaded:
+                    resolutions.append((path, zi, name, "provided", None))
+                    continue
+                how, found, fzi = self._find(name, path, chain)
+                if fzi is not None and id(fzi) in names:  # the same file by another name: one object
+                    names[id(fzi)].add(name)
+                    resolutions.append((path, zi, name, how, next(p for p, y in loaded if y is fzi)))
+                    continue
+                resolutions.append((path, zi, name, how, found))
+                if how == "provided":
+                    provided_loaded.add(name)
+                elif fzi is not None:
+                    loaded.append((found, fzi))
+                    names[id(fzi)] = {name, found}
+                    loader[id(fzi)] = zi
+        return loaded, resolutions, pending
+
+
+def check_with(zip_path, decoder, parser, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVIDED,
+               max_versions=None, ld_library_path=LAMBDA_LD_LIBRARY_PATH, batch_bytes=BATCH_BYTES):
+    """check_zip with the engines given (GpuUnzipDecoder and GpuElfParser, or stand-ins with the same interfaces)."""
+    if arch not in MACHINES:
+        raise ValueError("arch=%r: expected one of %s" % (arch, ", ".join(MACHINES)))
+    ceilings = {}
+    for prefix, v in (max_versions or {}).items():
+        if not re.fullmatch(r"\d+(?:\.\d+)*", str(v)):
+            raise ValueError("max_versions[%r]=%r: expected a dotted version such as 2.26" % (prefix, v))
+        ceilings[prefix] = _version_key(str(v))
+    with zipfile.ZipFile(zip_path) as zf, open(zip_path, "rb") as src:
+        src.seek(0, os.SEEK_END)
+        source = (zf, src, src.tell())
+        tree = _Tree(zf, mount)
+        path_of = {}
+        for p, zi in tree.files.items():
+            path_of.setdefault(id(zi), p)
+        roots = [(p, zi) for p, zi in sorted(tree.files.items()) if Z.selected_for_strip(zi)]
+        objs, rounds, uploaded = {}, 0, 0
+        model = _Model(tree, objs, arch, provided, ld_library_path)
+
+        def consume(part, decoded, whole):
+            refs = []
+            for key, zi, _ in part:
+                status, ref = decoded.get(key, (Z.UNZIP_OK, None))
+                if status != Z.UNZIP_OK:
+                    raise Z.BadZipMember(zi.filename, {Z.UNZIP_BAD_DATA: "Invalid DEFLATE data", Z.UNZIP_BAD_CRC: "Bad CRC-32",
+                                                       Z.UNZIP_WRONG_SIZE: "Wrong uncompressed size"}[status])
+                refs.append(ref if ref is not None else parser.upload(zf.read(zi)))
+            for (key, zi, _), (status, machine, records) in zip(part, parser.parse(refs)):
+                objs[id(zi)] = _Obj(zi, status, machine, records)
+
+        todo = [zi for _, zi in roots]
+        while todo:
+            rounds += 1
+            batch, cost = [], 0
+            for zi in todo:
+                c = zi.compress_size + 3 * zi.file_size + 1024
+                if batch and cost + c > batch_bytes:
+                    uploaded += Z.decode_members(decoder, batch, consume)
+                    batch, cost = [], 0
+                batch.append((id(zi), zi, source))
+                cost += c
+            if batch:
+                uploaded += Z.decode_members(decoder, batch, consume)
+            seen, todo = set(), []
+            for p, zi in roots:
+                for z in model.closure(p, zi)[2]:
+                    if id(z) not in objs and id(z) not in seen:
+                        seen.add(id(z))
+                        todo.append(z)
+        report = _report(tree, roots, objs, model, path_of, arch, ceilings)
+        report["stats"] = {"members": len(zf.infolist()), "roots": len(roots), "objects": len(objs), "rounds": rounds,
+                           "bytes_up": uploaded + parser.uploaded, "bytes_down": parser.downloaded,
+                           "inflate_ms": decoder.stats().get("kernel_ms", 0.0),
+                           "parse_ms": parser.stats().get("kernel_ms", 0.0)}
+    return report
+
+
+def _report(tree, roots, objs, model, path_of, arch, ceilings):
+    problems, notes, seen = [], [], set()
+    highest, provided_used = {}, {}
+
+    def problem(obj, kind, detail, weak=False):
+        key = (obj, kind, detail)
+        if key not in seen:
+            seen.add(key)
+            (notes if weak else problems).append({"object": obj, "kind": kind, "detail": detail})
+
+    objects, closures, resolved = {}, {}, {}
+    for zid, o in objs.items():
+        p = path_of[zid]
+        objects[p] = {"member": o.member.filename, "status": STATUS_NAMES.get(o.status, str(o.status)),
+                      "machine": o.machine, "soname": o.soname, "rpath": o.rpath, "runpath": o.runpath, "needed": None,
+                      "version_needs": [{"file": f, "version": v, "weak": w} for f, v, w in o.verneed],
+                      "version_defs": sorted(o.verdef)}
+    for root_path, root_zi in roots:
+        loaded, resolutions, _ = model.closure(root_path, root_zi)
+        closures[root_path] = [path_of[id(zi)] for _, zi in loaded]
+        by_name, filled = {}, set()  # names in this closure -> (how, path)
+        resolved[root_path] = [{"object": path_of[id(lzi)], "name": name, "how": how,
+                                "path": found and posixpath.normpath(found)} for _, lzi, name, how, found in resolutions]
+        for loader_path, lzi, name, how, found in resolutions:
+            by_name.setdefault(name, (how, found))
+            loader_path = posixpath.normpath(loader_path)
+            o = objects[path_of[id(lzi)]]
+            if o["needed"] is None:
+                o["needed"] = []
+                filled.add(id(lzi))
+            if id(lzi) in filled:
+                o["needed"].append({"name": name, "how": how, "path": found and posixpath.normpath(found)})
+            if how == "missing":
+                problem(loader_path, "missing", "%s: not in the zip, the search path or the runtime" % name)
+            elif how == "provided":
+                provided_used.setdefault(name, set()).add(loader_path)
+        filled = set()
+        for p, zi in loaded:
+            p = posixpath.normpath(p)
+            o = objs[id(zi)]
+            if o.status != N.ELF_OK:
+                problem(p, "unloadable", "%s: %s" % (o.member.filename, STATUS_NAMES.get(o.status, o.status)))
+                continue
+            if o.machine != MACHINES[arch]:
+                problem(p, "arch", "e_machine %d, not %s (%d)" % (o.machine, arch, MACHINES[arch]))
+            for f, v, weak in o.verneed:
+                how, found = by_name.get(f, (None, None))
+                if how == "provided":
+                    m = _VERSION.match(v)
+                    if m:
+                        prefix, key = m.group(1), _version_key(m.group(2))
+                        if prefix not in highest or key > _version_key(highest[prefix]):
+                            highest[prefix] = m.group(2)
+                        if prefix in ceilings and key > ceilings[prefix]:
+                            problem(p, "version", "%s from %s is newer than the runtime's %s_%s"
+                                    % (v, f, prefix, ".".join(map(str, ceilings[prefix]))), weak)
+                elif found is not None:
+                    t = objs.get(id(tree.lookup(found)))
+                    if t is not None and t.status == N.ELF_OK and v not in t.verdef:
+                        if not t.verdef:
+                            problem(p, "version", "%s: %s has no version information" % (v, f), True)
+                        else:
+                            problem(p, "version", "%s not defined by %s" % (v, f), weak)
+    return {"arch": arch, "mount": tree.mount, "objects": objects, "closures": closures, "resolved": resolved,
+            "problems": problems,
+            "notes": notes, "max_versions": dict(sorted(highest.items())),
+            "provided_used": {k: sorted(v) for k, v in sorted(provided_used.items())}}
+
+
+def check_zip(zip_path, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVIDED, max_versions=None,
+              ld_library_path=LAMBDA_LD_LIBRARY_PATH, ctx=None, batch_bytes=BATCH_BYTES):
+    """Check that the shared objects of `zip_path`, unpacked at `mount`, will load on Lambda (see the module docstring
+    for the search it restates).  Returns a plain dict:
+
+    * objects: {mounted path: member, status ("ok", "not ELF", "unsupported", "static", "malformed"), machine, soname,
+      rpath, runpath, needed [{name, how ("rpath", "ld_library_path", "runpath", "path", "loaded", "provided",
+      "missing"), path}] as the first root that loaded it resolved them, version_needs, version_defs};
+    * closures: {root: the members its dlopen loads (as keys of objects), in load order}; resolved: {root: every
+      need met in that load, [{object, name, how, path}] in the loader's order};
+    * problems [{object, kind, detail}]: kind "missing" (a DT_NEEDED resolved nowhere), "arch" (e_machine is not
+      `arch`'s: x86_64 62, arm64 183), "version" (a version need not defined by the member it resolved to, or above
+      the `max_versions` ceiling of its prefix on a provided library, such as {"GLIBC": "2.26"}), "unloadable" (a
+      loaded object that is not an ELF64 little-endian shared object with a dynamic section); weak version needs and
+      needs on members without version information go to notes instead;
+    * max_versions: the highest version needed of each prefix (GLIBC, GLIBCXX, CXXABI, GCC ...) on provided
+      libraries; provided_used: {soname: the objects whose need the `provided` list satisfied};
+    * stats: members, roots, objects (parsed), rounds, bytes_up, bytes_down, inflate_ms and parse_ms (CUDA events).
+
+    Members are inflated by the GPU zip reader and parsed on the GPU (lb2_elf_deps) where they lie; only the records
+    and their strings come back.  There is no CPU path: without a GPU this raises."""
+    from .tarball import _default_context
+    own = False
+    if ctx is None:
+        ctx, own = _default_context()
+    try:
+        with Z.GpuUnzipDecoder(ctx) as dec, GpuElfParser(ctx) as parser:
+            return check_with(zip_path, dec, parser, mount, arch, provided, max_versions, ld_library_path, batch_bytes)
+    finally:
+        if own:
+            ctx.close()
+
+
+def summary(report):
+    st = report["stats"]
+    lines = ["%d shared objects checked (%d roots, %d rounds) under %s for %s: %d problem(s)"
+             % (st["objects"], st["roots"], st["rounds"], report["mount"], report["arch"], len(report["problems"]))]
+    if report["max_versions"]:
+        lines.append("highest versions needed: " + ", ".join("%s_%s" % kv for kv in report["max_versions"].items()))
+    if report["provided_used"]:
+        lines.append("satisfied by the runtime list: " + ", ".join(report["provided_used"]))
+    for p in report["problems"]:
+        lines.append("problem: %s: %s: %s" % (p["object"], p["kind"], p["detail"]))
+    for p in report["notes"]:
+        lines.append("note: %s: %s: %s" % (p["object"], p["kind"], p["detail"]))
+    return "\n".join(lines)
+
+
+def _ceiling(text):
+    m = _VERSION.match(text)
+    if not m:
+        raise ValueError("--max-version %r: expected PREFIX_VERSION such as GLIBC_2.26" % text)
+    return m.group(1), m.group(2)
+
+
+def main(argv=None, check=check_zip):
+    """exit status 0: no problem; 1: problems; 2: a refused input or a usage error"""
+    import argparse
+    ap = argparse.ArgumentParser(prog="python -m lambdipy_b200.deps",
+                                 description="check that the shared objects of a Lambda zip will load there")
+    ap.add_argument("zip")
+    ap.add_argument("--mount", default="/var/task", help="where the zip is unpacked: /var/task (function) or /opt (layer)")
+    ap.add_argument("--arch", choices=sorted(MACHINES), default="x86_64")
+    ap.add_argument("--provided", action="append", metavar="NAME",
+                    help="a soname the runtime supplies (repeatable; replaces the default list)")
+    ap.add_argument("--max-version", action="append", default=[], metavar="PREFIX_VERSION",
+                    help="the runtime's highest version of a prefix, such as GLIBC_2.26 (repeatable)")
+    ap.add_argument("--ld-library-path", default=LAMBDA_LD_LIBRARY_PATH)
+    ap.add_argument("--json", action="store_true", help="print the whole report as JSON")
+    args = ap.parse_args(argv)
+    try:
+        ceilings = dict(_ceiling(t) for t in args.max_version)
+        report = check(args.zip, mount=args.mount, arch=args.arch,
+                       provided=DEFAULT_PROVIDED if args.provided is None else frozenset(args.provided),
+                       max_versions=ceilings, ld_library_path=args.ld_library_path)
+    except (OSError, ValueError, zipfile.BadZipFile) as e:
+        print("error: %s" % e, file=sys.stderr)
+        return 2
+    print(json.dumps(report, indent=1, sort_keys=True) if args.json else summary(report))
+    return 1 if report["problems"] else 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

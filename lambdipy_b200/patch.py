@@ -20,6 +20,12 @@ With LAMBDIPY_BUNDLE_VERIFY=1 (default: unset, nothing changes) and LAMBDIPY_BUN
 read back on the GPU (zipfile_gpu.testzip: every member inflated and CRC-checked) before the size line; a bad member
 fails the build, and the line gains the member count.  No other value is accepted.
 
+With LAMBDIPY_BUNDLE_CHECK_DEPS=1 (default: unset, nothing changes) and LAMBDIPY_BUNDLE_ZIP set, the written bundle's
+shared objects are checked on the GPU for what they need at load time (deps.check_zip at /var/task: every DT_NEEDED
+found in the bundle or the runtime, the architecture, the symbol versions) after the zip and after
+LAMBDIPY_BUNDLE_VERIFY's read-back; a problem fails the build, and the size line gains the count of objects checked.
+No other value is accepted.
+
 With LAMBDIPY_DEFLATE_LEVEL=9 (default: unset, the default encoder) the GPU tarball mirror and the bundle zip use
 the thorough encoder (an optimal parse; smaller output, longer kernels).  No other value is accepted.
 
@@ -67,6 +73,16 @@ def bundle_verify():
     return True
 
 
+def bundle_check_deps():
+    """LAMBDIPY_BUNDLE_CHECK_DEPS, checked: False when unset, True for 1."""
+    v = os.environ.get("LAMBDIPY_BUNDLE_CHECK_DEPS")
+    if v is None:
+        return False
+    if v != "1":
+        raise ValueError("LAMBDIPY_BUNDLE_CHECK_DEPS=%r: expected 1 (check the bundle's shared objects on the GPU) or unset" % v)
+    return True
+
+
 def seek_table():
     """LAMBDIPY_SEEK_TABLE, checked: False when unset, True for 1."""
     v = os.environ.get("LAMBDIPY_SEEK_TABLE")
@@ -77,9 +93,9 @@ def seek_table():
     return True
 
 
-def zip_after_copy(copy_include_paths, zip_path, compresslevel=None, verify=False, seek=False):
-    """copy_include_paths followed by the bundle zip of its build directory, with verify its read-back check, and the
-    size line."""
+def zip_after_copy(copy_include_paths, zip_path, compresslevel=None, verify=False, seek=False, check_deps=False):
+    """copy_include_paths followed by the bundle zip of its build directory, with verify its read-back check, with
+    check_deps the load-time check of its shared objects (deps.check_zip), and the size line."""
     def wrapped(include_paths, build_directory="./build"):
         copy_include_paths(include_paths, build_directory)
         from . import project_build, zipfile_gpu
@@ -93,6 +109,12 @@ def zip_after_copy(copy_include_paths, zip_path, compresslevel=None, verify=Fals
                 raise RuntimeError("bundle zip %s: member %r does not read back (bad data, size or CRC-32)" % (zip_path, bad))
             with zipfile.ZipFile(zip_path) as zf:
                 checked = "; %d members checked" % len(zf.infolist())
+        if check_deps:
+            from . import deps
+            report = deps.check_zip(zip_path)
+            if report["problems"]:
+                raise RuntimeError("bundle zip %s: shared objects that will not load:\n%s" % (zip_path, deps.summary(report)))
+            checked += "; %d shared objects checked" % report["stats"]["objects"]
         zipped, unzipped = os.path.getsize(zip_path), project_build.tree_bytes(build_directory)
         print("Bundle zip: %s, %.1f MB = %.0f %% of the 50 MB direct-upload limit; unzipped %.1f MB = %.0f %% of 250 MB%s"
               % (zip_path, zipped / 1e6, 100.0 * zipped / LAMBDA_ZIPPED_LIMIT, unzipped / 1e6,
@@ -110,6 +132,7 @@ def apply():
     zip_path = bundle_zip_path()
     level = deflate_level()
     verify = bundle_verify()
+    check_deps = bundle_check_deps()
     seek = seek_table()
     import lambdipy.cli as cli
     import lambdipy.project_build as ref
@@ -125,7 +148,8 @@ def apply():
         from . import tarball
         ref.prepare_tarfile = tarball.prepare_tarfile
     if zip_path is not None:
-        cli.copy_include_paths = zip_after_copy(ref.copy_include_paths, zip_path, level, verify=verify, seek=seek)
+        cli.copy_include_paths = zip_after_copy(ref.copy_include_paths, zip_path, level, verify=verify, seek=seek,
+                                               check_deps=check_deps)
     # `lambdipy build` spends seconds resolving, downloading and copying packages before it reaches the
     # strip step (cli.py:52-67): create the CUDA context behind that, not in front of the strip
     if os.environ.get("LAMBDIPY_B200_EAGER_WARMUP", "1") != "0":
