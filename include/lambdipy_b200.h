@@ -538,6 +538,68 @@ int lb2_elf_deps(lb2_ctx *ctx, const uint64_t *d_ptrs, const uint64_t *sizes, ui
                  lb2_elf_record *records, uint32_t max_records, uint32_t *n_records, void *h_pool, uint64_t pool_cap,
                  uint64_t *pool_bytes, lb2_elf_deps_stats *stats);
 
+/* ---- symbol lookups: the undefined symbols a shared object binds when it is loaded ---------------------------- */
+/* What ld.so's relocation of an object looks up (glibc elf/dl-lookup.c do_lookup_x and check_match), done for many
+ * objects at once, which is how deps.check_zip(symbols=True) finds the "undefined symbol" a dlopen would fail on.
+ * A resolver (lb2_syms) owns a device arena that outlives the objects it indexed.
+ *
+ * lb2_syms_index: objects i < n lie at the device addresses d_ptrs[i] (sizes[i] bytes; both arrays in host memory;
+ * any alignment).  One warp per object reads its dynamic array, copies .dynsym, .dynstr, .gnu.version, its hash table
+ * (DT_GNU_HASH, else DT_HASH) and its version table into the arena, and lists its references: the symbols that a
+ * DT_RELA or DT_JMPREL entry names which are SHN_UNDEF and not STB_LOCAL.  ids[i] receives the object's id in the
+ * resolver, objects[i] its status (LB2_SYM_*) and counts.  No byte outside an object's [0, size) is read, and the
+ * object may be freed when the call returns.  LB2_E_CAPACITY when the arena cannot grow (nothing was added).
+ *
+ * lb2_syms_resolve: job j looks up every reference of object jobs[j].obj in the scope scope[scope_off ..+ scope_len)
+ * (object ids, in lookup order), one warp per (reference, job).  counts[3 j + classes[id]] counts the references the
+ * object `id` defined first in scope order (classes: one byte per id, 0 .. 2).  A strong reference defined nowhere is
+ * a miss {job, ref}, in no particular order; *n_misses says how many there were, LB2_E_CAPACITY when more than
+ * max_misses (counts are then complete).  Weak references found nowhere are counted nowhere.
+ *
+ * lb2_syms_names: the strings of misses[0 .. n): for miss i, h_pool[offsets[i] ..] holds its symbol name, the name of
+ * the version it asks for and the file of that version need, each followed by a NUL (empty when not versioned).
+ * LB2_E_CAPACITY when pool_cap is too small (*pool_bytes says what is needed). */
+#define LB2_SYM_OK 0
+#define LB2_SYM_NOT_ELF 1
+#define LB2_SYM_UNSUPPORTED 2        /* ELF32, big-endian, or DT_REL relocations                                     */
+#define LB2_SYM_STATIC 3
+#define LB2_SYM_MALFORMED 4          /* elf_deps' bounds rules, a hash table or a relocation symbol index outside its */
+                                     /* table, DT_SYMENT != 24, DT_RELAENT != 24, a reference name not ended          */
+typedef struct lb2_syms lb2_syms;
+typedef struct lb2_sym_object {
+  int32_t status;                    /* LB2_SYM_*                                                                  */
+  uint32_t flags;                    /* 1: DT_GNU_HASH, 2: DT_HASH, 4: DT_VERSYM                                   */
+  uint32_t nsyms, nver;              /* symbols copied (the hash table's, or past it up to the top relocation's)   */
+  uint32_t nbucket, symoffset, bloom_words, bloom_shift;
+  uint32_t nrefs, nhash;             /* references; symbols the hash table covers                                   */
+  uint64_t str_len, hash_len;
+  uint64_t sym_off, str_off, versym_off, hash_off;
+  uint64_t rela_off, rela_n, plt_off, plt_n;
+  uint64_t arena, refs;              /* device addresses of its tables and references                              */
+} lb2_sym_object;
+typedef struct lb2_sym_job {
+  uint32_t obj, scope_off, scope_len, pad;
+} lb2_sym_job;
+typedef struct lb2_sym_miss {
+  uint32_t job, ref;
+} lb2_sym_miss;
+typedef struct lb2_syms_stats {
+  uint64_t bytes_up, bytes_down;     /* host-device bytes of the call                                              */
+  uint64_t references, lookups;      /* references indexed or resolved; scope entries probed                        */
+  uint64_t arena_bytes;              /* the arena's size after the call                                            */
+  float index_ms, refs_ms, resolve_ms; /* kernels (CUDA events)                                                    */
+  float pad;
+} lb2_syms_stats;
+int lb2_syms_create(lb2_ctx *ctx, lb2_syms **out);
+void lb2_syms_destroy(lb2_syms *s);
+int lb2_syms_index(lb2_syms *s, const uint64_t *d_ptrs, const uint64_t *sizes, uint32_t n, uint32_t *ids,
+                   lb2_sym_object *objects, lb2_syms_stats *stats);
+int lb2_syms_resolve(lb2_syms *s, const lb2_sym_job *jobs, uint32_t n_jobs, const uint32_t *scope, uint32_t n_scope,
+                     const uint8_t *classes, uint32_t *counts, lb2_sym_miss *misses, uint32_t max_misses,
+                     uint32_t *n_misses, lb2_syms_stats *stats);
+int lb2_syms_names(lb2_syms *s, const lb2_sym_job *jobs, uint32_t n_jobs, const lb2_sym_miss *misses, uint32_t n,
+                   uint64_t *offsets, void *h_pool, uint64_t pool_cap, uint64_t *pool_bytes, lb2_syms_stats *stats);
+
 #ifdef __cplusplus
 }
 #endif

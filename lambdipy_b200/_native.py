@@ -32,12 +32,14 @@ EXPORTS = [
     "lb2_inflate_device_output", "lb2_memcpy_d2d", "lb2_gzip_submit_device", "lb2_tar_index",
     "lb2_gzip_chunk_sizes", "lb2_inflate_run_table", "lb2_zip_chunk_sizes", "lb2_unzip_run_table",
     "lb2_cleanup_tests_removed", "lb2_elf_deps",
+    "lb2_syms_create", "lb2_syms_destroy", "lb2_syms_index", "lb2_syms_resolve", "lb2_syms_names",
 ]
 TAR_STOP_ZERO, TAR_STOP_BAD_HEADER, TAR_STOP_END, TAR_STOP_UNSUPPORTED = 1, 2, 3, 4
 ZIP_CONTINUES, ZIP_MORE = 1, 2
 ELF_OK, ELF_NOT_ELF, ELF_UNSUPPORTED, ELF_STATIC, ELF_MALFORMED = 0, 1, 2, 3, 4  # LB2_ELF_*
 ELF_REC_SONAME, ELF_REC_NEEDED, ELF_REC_RPATH, ELF_REC_RUNPATH = 1, 2, 3, 4  # LB2_ELF_REC_*
 ELF_REC_VERNEED_FILE, ELF_REC_VERNEED_VERSION, ELF_REC_VERDEF = 5, 6, 7
+SYM_OK, SYM_UNSUPPORTED, SYM_MALFORMED = 0, 2, 4  # LB2_SYM_* (the LB2_ELF_* values)
 DEFLATE_BEST = 1  # LB2_DEFLATE_BEST
 
 
@@ -175,6 +177,34 @@ class ElfDepsStats(C.Structure):
 
     def as_dict(self):
         return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class SymObject(C.Structure):
+    _fields_ = [("status", C.c_int32), ("flags", C.c_uint32), ("nsyms", C.c_uint32), ("nver", C.c_uint32),
+                ("nbucket", C.c_uint32), ("symoffset", C.c_uint32), ("bloom_words", C.c_uint32),
+                ("bloom_shift", C.c_uint32), ("nrefs", C.c_uint32), ("nhash", C.c_uint32), ("str_len", C.c_uint64),
+                ("hash_len", C.c_uint64), ("sym_off", C.c_uint64), ("str_off", C.c_uint64), ("versym_off", C.c_uint64),
+                ("hash_off", C.c_uint64), ("rela_off", C.c_uint64), ("rela_n", C.c_uint64), ("plt_off", C.c_uint64),
+                ("plt_n", C.c_uint64), ("arena", C.c_uint64), ("refs", C.c_uint64)]
+
+
+class SymRef(C.Structure):  # elf_syms.cuh Ref: a reference as the arena holds it
+    _fields_ = [("sym", C.c_uint32), ("name", C.c_uint32), ("name_len", C.c_uint32), ("gnu", C.c_uint32),
+                ("sysv", C.c_uint32), ("ver", C.c_uint16), ("weak", C.c_uint8), ("pad", C.c_uint8)]
+
+
+class SymJob(C.Structure):
+    _fields_ = [("obj", C.c_uint32), ("scope_off", C.c_uint32), ("scope_len", C.c_uint32), ("pad", C.c_uint32)]
+
+
+class SymMiss(C.Structure):
+    _fields_ = [("job", C.c_uint32), ("ref", C.c_uint32)]
+
+
+class SymsStats(C.Structure):
+    _fields_ = [("bytes_up", C.c_uint64), ("bytes_down", C.c_uint64), ("references", C.c_uint64),
+                ("lookups", C.c_uint64), ("arena_bytes", C.c_uint64), ("index_ms", C.c_float),
+                ("refs_ms", C.c_float), ("resolve_ms", C.c_float), ("pad", C.c_float)]
 
 
 class FillRegion(C.Structure):
@@ -316,6 +346,18 @@ def load():
     lib.lb2_elf_deps.argtypes = [vp, u64p, u64p, C.c_uint32, C.POINTER(ElfObject), C.POINTER(ElfRecord), C.c_uint32,
                                  u32p, vp, C.c_uint64, u64p, C.POINTER(ElfDepsStats)]
     lib.lb2_elf_deps.restype = C.c_int
+    lib.lb2_syms_create.argtypes = [vp, C.POINTER(vp)]
+    lib.lb2_syms_create.restype = C.c_int
+    lib.lb2_syms_destroy.argtypes = [vp]
+    lib.lb2_syms_destroy.restype = None
+    lib.lb2_syms_index.argtypes = [vp, u64p, u64p, C.c_uint32, u32p, C.POINTER(SymObject), C.POINTER(SymsStats)]
+    lib.lb2_syms_index.restype = C.c_int
+    lib.lb2_syms_resolve.argtypes = [vp, C.POINTER(SymJob), C.c_uint32, u32p, C.c_uint32, C.POINTER(C.c_uint8), u32p,
+                                     C.POINTER(SymMiss), C.c_uint32, u32p, C.POINTER(SymsStats)]
+    lib.lb2_syms_resolve.restype = C.c_int
+    lib.lb2_syms_names.argtypes = [vp, C.POINTER(SymJob), C.c_uint32, C.POINTER(SymMiss), C.c_uint32, u64p, vp,
+                                   C.c_uint64, u64p, C.POINTER(SymsStats)]
+    lib.lb2_syms_names.restype = C.c_int
     _lib = lib
     return lib
 

@@ -6,8 +6,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "liblambdipy_b200.so")
-SOURCES = ["strip_host.cu", "strip_tree.cu", "plan.cu", "compact.cu", "compact_tma.cu", "corpus.cu", "deflate.cu", "inflate.cu", "tar.cu", "elf_deps.cu", "api.cu"]
-HEADERS = ["lb2_common.cuh", "lb2_host.cuh", "copy_device.cuh", "inflate_core.cuh", "deflate_parse.cuh", "tar_walk.cuh", "elf_deps.cuh", os.path.join("..", "..", "include", "lambdipy_b200.h")]
+SOURCES = ["strip_host.cu", "strip_tree.cu", "plan.cu", "compact.cu", "compact_tma.cu", "corpus.cu", "deflate.cu", "inflate.cu", "tar.cu", "elf_deps.cu", "elf_syms.cu", "api.cu"]
+HEADERS = ["lb2_common.cuh", "lb2_host.cuh", "copy_device.cuh", "inflate_core.cuh", "deflate_parse.cuh", "tar_walk.cuh", "elf_deps.cuh", "elf_syms.cuh", os.path.join("..", "..", "include", "lambdipy_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-Wall,-Wno-unused-function", "--shared", "-cudart", "shared",

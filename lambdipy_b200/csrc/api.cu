@@ -1733,3 +1733,302 @@ int lb2_elf_deps(lb2_ctx *ctx, const uint64_t *d_ptrs, const uint64_t *sizes, ui
 }
 
 }  // extern "C"
+
+// ---------------------------------------------------------------------------- symbol lookups
+// The index, reference and resolve kernels (elf_syms.cu) on the context's stream.  The arena is a list of device
+// chunks; an index call takes one block for the tables of its batch and one for their references, each object's
+// pieces at 8-byte alignment.  Scratch of a call lives in one allocation freed before it returns.
+#include "elf_syms.cuh"
+static_assert(sizeof(lb2_sym_object) == sizeof(elfs::Object), "the index kernels write lb2_sym_object records");
+static_assert(sizeof(lb2_sym_job) == sizeof(elfs::Job) && sizeof(lb2_sym_miss) == sizeof(elfs::Miss), "resolve records");
+
+struct lb2_syms {
+  lb2_ctx *ctx = nullptr;
+  std::vector<void *> chunks;
+  uint8_t *cur = nullptr;
+  uint64_t used = 0, cap = 0, total = 0;
+  std::vector<lb2_sym_object> objs;
+};
+
+namespace {
+constexpr uint64_t SYM_CHUNK = 64ull << 20;
+
+// n bytes of the arena (8-aligned), or nullptr when the device has no room for a new chunk
+uint8_t *syms_alloc(lb2_syms *s, uint64_t n) {
+  n = (n + 255) & ~255ull;
+  if (!n) return nullptr;
+  if (s->used + n > s->cap) {
+    const uint64_t c = n > SYM_CHUNK ? n : SYM_CHUNK;
+    void *p = nullptr;
+    if (cudaMalloc(&p, c) != cudaSuccess) {
+      cudaGetLastError();
+      return nullptr;
+    }
+    s->chunks.push_back(p);
+    s->cur = static_cast<uint8_t *>(p);
+    s->used = 0;
+    s->cap = c;
+    s->total += c;
+  }
+  uint8_t *p = s->cur + s->used;
+  s->used += n;
+  return p;
+}
+
+struct SymScratch {  // one device allocation and the events of a call
+  uint8_t *d = nullptr;
+  cudaEvent_t ev[8] = {};
+  cudaError_t e = cudaSuccess;
+  explicit SymScratch(uint64_t bytes) {
+    e = cudaMalloc(&d, bytes ? bytes : 16);
+    for (auto &v : ev)
+      if (e == cudaSuccess) e = cudaEventCreate(&v);
+  }
+  float ms(int a, int b) {
+    float t = 0;
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&t, ev[a], ev[b]);
+    return t;
+  }
+  ~SymScratch() {
+    cudaFree(d);
+    for (auto &v : ev) if (v) cudaEventDestroy(v);
+  }
+};
+}  // namespace
+
+extern "C" {
+
+int lb2_syms_create(lb2_ctx *ctx, lb2_syms **out) {
+  if (!ctx) return LB2_E_ARG;
+  if (!out) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  *out = new lb2_syms;
+  (*out)->ctx = ctx;
+  return LB2_OK;
+}
+
+void lb2_syms_destroy(lb2_syms *s) {
+  if (!s) return;
+  cudaSetDevice(s->ctx->device);
+  for (void *p : s->chunks) cudaFree(p);
+  delete s;
+}
+
+int lb2_syms_index(lb2_syms *s, const uint64_t *d_ptrs, const uint64_t *sizes, uint32_t n, uint32_t *ids,
+                   lb2_sym_object *objects, lb2_syms_stats *stats) {
+  if (!s) return LB2_E_ARG;
+  lb2_ctx *ctx = s->ctx;
+  if (n && (!d_ptrs || !sizes || !ids || !objects)) { ctx->err = "NULL argument"; return LB2_E_ARG; }
+  for (uint32_t i = 0; i < n; i++)
+    if (!d_ptrs[i] && sizes[i]) { ctx->err = "lb2_syms_index: a NULL object address"; return LB2_E_ARG; }
+  lb2_syms_stats st{};
+  if (!n) { if (stats) *stats = st; return LB2_OK; }
+  CK(cudaSetDevice(ctx->device));
+  const uint64_t job_bytes = 2 * sizeof(uint64_t) * (uint64_t)n, obj_bytes = sizeof(lb2_sym_object) * (uint64_t)n;
+  SymScratch w(job_bytes + obj_bytes + 8 * ((uint64_t)n + 1));
+  cudaError_t &e = w.e;
+  const uint64_t *d_p = reinterpret_cast<const uint64_t *>(w.d), *d_s = d_p + n;
+  void *d_obj = w.d + job_bytes;
+  uint64_t *d_base = reinterpret_cast<uint64_t *>(w.d + job_bytes + obj_bytes);
+  cudaStream_t q = ctx->stream;
+  if (e == cudaSuccess) e = cudaMemcpyAsync(w.d, d_ptrs, job_bytes / 2, cudaMemcpyHostToDevice, q);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(w.d + job_bytes / 2, sizes, job_bytes / 2, cudaMemcpyHostToDevice, q);
+  if (e == cudaSuccess) e = cudaEventRecord(w.ev[0], q);
+  if (e == cudaSuccess) { launch_syms_index_count(d_p, d_s, n, d_obj, q); e = cudaGetLastError(); }
+  if (e == cudaSuccess) e = cudaEventRecord(w.ev[1], q);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(objects, d_obj, obj_bytes, cudaMemcpyDeviceToHost, q);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(q);
+  st.bytes_up += job_bytes;
+  st.bytes_down += obj_bytes;
+  // the tables' block, and the relocation entries' prefix
+  std::vector<uint64_t> base(n + 1, 0);
+  uint64_t need = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    base[i + 1] = base[i] + (objects[i].status == elfs::ST_OK ? objects[i].rela_n + objects[i].plt_n : 0);
+    if (objects[i].status == elfs::ST_OK) need += elfs::tables(reinterpret_cast<const elfs::Object &>(objects[i])).end;
+  }
+  uint8_t *block = nullptr;
+  if (e == cudaSuccess && need) {
+    block = syms_alloc(s, need);
+    if (!block) { ctx->err = "lb2_syms_index: no device memory for the symbol arena"; return LB2_E_CAPACITY; }
+    uint64_t at = 0;
+    for (uint32_t i = 0; i < n; i++)
+      if (objects[i].status == elfs::ST_OK) {
+        objects[i].arena = reinterpret_cast<uint64_t>(block + at);
+        at += elfs::tables(reinterpret_cast<const elfs::Object &>(objects[i])).end;
+      }
+    e = cudaMemsetAsync(block, 0, need, q);
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_obj, objects, obj_bytes, cudaMemcpyHostToDevice, q);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_base, base.data(), 8 * ((uint64_t)n + 1), cudaMemcpyHostToDevice, q);
+  st.bytes_up += obj_bytes + 8 * ((uint64_t)n + 1);
+  if (e == cudaSuccess) e = cudaEventRecord(w.ev[2], q);
+  if (e == cudaSuccess) { launch_syms_index_write(d_p, d_s, n, d_obj, q); e = cudaGetLastError(); }
+  if (e == cudaSuccess) e = cudaEventRecord(w.ev[3], q);
+  if (e == cudaSuccess) { launch_syms_refs(d_p, d_base, base[n], n, d_obj, q); e = cudaGetLastError(); }
+  if (e == cudaSuccess) e = cudaEventRecord(w.ev[4], q);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(objects, d_obj, obj_bytes, cudaMemcpyDeviceToHost, q);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(q);
+  st.bytes_down += obj_bytes;
+  uint64_t nrefs = 0;
+  for (uint32_t i = 0; i < n; i++) nrefs += objects[i].nrefs;
+  if (e == cudaSuccess && nrefs) {
+    uint8_t *refs = syms_alloc(s, nrefs * sizeof(elfs::Ref));
+    if (!refs) { ctx->err = "lb2_syms_index: no device memory for the symbol arena"; return LB2_E_CAPACITY; }
+    uint64_t at = 0;
+    for (uint32_t i = 0; i < n; i++) {
+      objects[i].refs = objects[i].nrefs ? reinterpret_cast<uint64_t>(refs + at) : 0;
+      at += objects[i].nrefs * sizeof(elfs::Ref);
+    }
+    e = cudaMemcpyAsync(d_obj, objects, obj_bytes, cudaMemcpyHostToDevice, q);
+    st.bytes_up += obj_bytes;
+    if (e == cudaSuccess) e = cudaEventRecord(w.ev[5], q);
+    if (e == cudaSuccess) { launch_syms_refs_write(n, d_obj, q); e = cudaGetLastError(); }
+    if (e == cudaSuccess) e = cudaEventRecord(w.ev[6], q);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(q);
+    st.refs_ms += w.ms(5, 6);
+  }
+  st.index_ms += w.ms(0, 1) + w.ms(2, 3);
+  st.refs_ms += w.ms(3, 4);
+  if (e != cudaSuccess) { ctx->err = std::string("lb2_syms_index: ") + cudaGetErrorString(e); return LB2_E_CUDA; }
+  for (uint32_t i = 0; i < n; i++) {
+    ids[i] = (uint32_t)s->objs.size();
+    s->objs.push_back(objects[i]);
+  }
+  st.references = nrefs;
+  st.arena_bytes = s->total;
+  if (stats) *stats = st;
+  return LB2_OK;
+}
+
+int lb2_syms_resolve(lb2_syms *s, const lb2_sym_job *jobs, uint32_t n_jobs, const uint32_t *scope, uint32_t n_scope,
+                     const uint8_t *classes, uint32_t *counts, lb2_sym_miss *misses, uint32_t max_misses,
+                     uint32_t *n_misses, lb2_syms_stats *stats) {
+  if (!s) return LB2_E_ARG;
+  lb2_ctx *ctx = s->ctx;
+  const uint64_t n_obj = s->objs.size();
+  if ((n_jobs && (!jobs || !counts)) || (n_scope && !scope) || (n_obj && !classes) || !n_misses || (max_misses && !misses)) {
+    ctx->err = "NULL argument";
+    return LB2_E_ARG;
+  }
+  for (uint32_t i = 0; i < n_scope; i++)
+    if (scope[i] >= n_obj) { ctx->err = "lb2_syms_resolve: a scope entry is not an object id"; return LB2_E_ARG; }
+  for (uint64_t i = 0; i < n_obj; i++)
+    if (classes[i] > 2) { ctx->err = "lb2_syms_resolve: a class above 2"; return LB2_E_ARG; }
+  std::vector<uint64_t> base(n_jobs + 1, 0);
+  for (uint32_t j = 0; j < n_jobs; j++) {
+    if (jobs[j].obj >= n_obj || jobs[j].scope_off > n_scope || jobs[j].scope_len > n_scope - jobs[j].scope_off) {
+      ctx->err = "lb2_syms_resolve: a job outside the objects or the scope array";
+      return LB2_E_ARG;
+    }
+    base[j + 1] = base[j] + s->objs[jobs[j].obj].nrefs;
+  }
+  lb2_syms_stats st{};
+  *n_misses = 0;
+  if (n_jobs) memset(counts, 0, 12ull * n_jobs);
+  if (!n_jobs) { if (stats) *stats = st; return LB2_OK; }
+  CK(cudaSetDevice(ctx->device));
+  const uint64_t ob = sizeof(lb2_sym_object) * n_obj, jb = sizeof(lb2_sym_job) * n_jobs, bb = 8 * ((uint64_t)n_jobs + 1),
+                 sb = 4ull * n_scope, cb = 12ull * n_jobs, mb = sizeof(lb2_sym_miss) * (uint64_t)max_misses;
+  uint64_t o[8] = {0};  // offsets: objects, jobs, base, scope, classes, counts + n_miss + lookups, misses, end
+  const uint64_t sz[7] = {ob, jb, bb, sb, n_obj, cb + 16, mb};
+  for (int k = 0; k < 7; k++) o[k + 1] = (o[k] + sz[k] + 15) & ~15ull;
+  SymScratch w(o[7]);
+  cudaError_t &e = w.e;
+  cudaStream_t q = ctx->stream;
+  const void *src[5] = {s->objs.data(), jobs, base.data(), scope, classes};
+  for (int k = 0; k < 5; k++)
+    if (e == cudaSuccess && sz[k]) e = cudaMemcpyAsync(w.d + o[k], src[k], sz[k], cudaMemcpyHostToDevice, q);
+  if (e == cudaSuccess) e = cudaMemsetAsync(w.d + o[5], 0, cb + 16, q);
+  st.bytes_up = ob + jb + bb + sb + n_obj;
+  uint32_t *d_counts = reinterpret_cast<uint32_t *>(w.d + o[5]), *d_nmiss = d_counts + 3ull * n_jobs;
+  unsigned long long *d_lookups = reinterpret_cast<unsigned long long *>(w.d + ((o[5] + cb + 4 + 7) & ~7ull));
+  if (e == cudaSuccess) e = cudaEventRecord(w.ev[0], q);
+  if (e == cudaSuccess) {
+    launch_syms_resolve(w.d + o[0], reinterpret_cast<const elfs::Job *>(w.d + o[1]), reinterpret_cast<const uint64_t *>(w.d + o[2]),
+                        n_jobs, base[n_jobs], reinterpret_cast<const uint32_t *>(w.d + o[3]), w.d + o[4], d_counts,
+                        reinterpret_cast<elfs::Miss *>(w.d + o[6]), max_misses, d_nmiss, d_lookups, q);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaEventRecord(w.ev[1], q);
+  unsigned long long lookups = 0;
+  if (e == cudaSuccess) e = cudaMemcpyAsync(counts, d_counts, cb, cudaMemcpyDeviceToHost, q);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(n_misses, d_nmiss, 4, cudaMemcpyDeviceToHost, q);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&lookups, d_lookups, 8, cudaMemcpyDeviceToHost, q);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(q);
+  st.bytes_down = cb + 12;
+  const uint32_t got = *n_misses < max_misses ? *n_misses : max_misses;
+  if (e == cudaSuccess && got) e = cudaMemcpy(misses, w.d + o[6], sizeof(lb2_sym_miss) * (uint64_t)got, cudaMemcpyDeviceToHost);
+  st.bytes_down += sizeof(lb2_sym_miss) * (uint64_t)got;
+  st.resolve_ms = w.ms(0, 1);
+  if (e != cudaSuccess) { ctx->err = std::string("lb2_syms_resolve: ") + cudaGetErrorString(e); return LB2_E_CUDA; }
+  st.references = base[n_jobs];
+  st.lookups = lookups;
+  st.arena_bytes = s->total;
+  if (stats) *stats = st;
+  if (*n_misses > max_misses) { ctx->err = "lb2_syms_resolve: more misses than max_misses (*n_misses needed)"; return LB2_E_CAPACITY; }
+  return LB2_OK;
+}
+
+int lb2_syms_names(lb2_syms *s, const lb2_sym_job *jobs, uint32_t n_jobs, const lb2_sym_miss *misses, uint32_t n,
+                   uint64_t *offsets, void *h_pool, uint64_t pool_cap, uint64_t *pool_bytes, lb2_syms_stats *stats) {
+  if (!s) return LB2_E_ARG;
+  lb2_ctx *ctx = s->ctx;
+  if ((n_jobs && !jobs) || (n && (!misses || !offsets)) || !pool_bytes || (pool_cap && !h_pool)) {
+    ctx->err = "NULL argument";
+    return LB2_E_ARG;
+  }
+  for (uint32_t j = 0; j < n_jobs; j++)
+    if (jobs[j].obj >= s->objs.size()) { ctx->err = "lb2_syms_names: a job outside the objects"; return LB2_E_ARG; }
+  for (uint32_t i = 0; i < n; i++)
+    if (misses[i].job >= n_jobs || misses[i].ref >= s->objs[jobs[misses[i].job].obj].nrefs) {
+      ctx->err = "lb2_syms_names: a miss outside its job's references";
+      return LB2_E_ARG;
+    }
+  lb2_syms_stats st{};
+  *pool_bytes = 0;
+  if (!n) { if (stats) *stats = st; return LB2_OK; }
+  CK(cudaSetDevice(ctx->device));
+  const uint64_t ob = sizeof(lb2_sym_object) * s->objs.size(), jb = sizeof(lb2_sym_job) * n_jobs,
+                 mb = sizeof(lb2_sym_miss) * (uint64_t)n, lb = 8ull * n;
+  const uint64_t o1 = (ob + 15) & ~15ull, o2 = (o1 + jb + 15) & ~15ull, o3 = (o2 + mb + 15) & ~15ull, o4 = o3 + lb;
+  SymScratch w(o4);
+  cudaError_t &e = w.e;
+  cudaStream_t q = ctx->stream;
+  if (e == cudaSuccess) e = cudaMemcpyAsync(w.d, s->objs.data(), ob, cudaMemcpyHostToDevice, q);
+  if (e == cudaSuccess && jb) e = cudaMemcpyAsync(w.d + o1, jobs, jb, cudaMemcpyHostToDevice, q);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(w.d + o2, misses, mb, cudaMemcpyHostToDevice, q);
+  uint64_t *d_len = reinterpret_cast<uint64_t *>(w.d + o3);
+  const elfs::Job *d_jobs = reinterpret_cast<const elfs::Job *>(w.d + o1);
+  const elfs::Miss *d_miss = reinterpret_cast<const elfs::Miss *>(w.d + o2);
+  if (e == cudaSuccess) { launch_syms_names(w.d, d_jobs, d_miss, n, d_len, nullptr, q); e = cudaGetLastError(); }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(offsets, d_len, lb, cudaMemcpyDeviceToHost, q);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(q);
+  st.bytes_up += ob + jb + mb;
+  st.bytes_down += lb;
+  uint64_t total = 0;
+  if (e == cudaSuccess)
+    for (uint32_t i = 0; i < n; i++) {
+      const uint64_t l = offsets[i];
+      offsets[i] = total;
+      total += l;
+    }
+  *pool_bytes = total;
+  const bool fits = total <= pool_cap;
+  uint8_t *d_pool = nullptr;
+  if (e == cudaSuccess && fits) e = cudaMalloc(&d_pool, total);
+  if (e == cudaSuccess && fits) e = cudaMemcpyAsync(d_len, offsets, lb, cudaMemcpyHostToDevice, q);
+  if (e == cudaSuccess && fits) { launch_syms_names(w.d, d_jobs, d_miss, n, d_len, d_pool, q); e = cudaGetLastError(); }
+  if (e == cudaSuccess && fits) e = cudaMemcpyAsync(h_pool, d_pool, total, cudaMemcpyDeviceToHost, q);
+  if (e == cudaSuccess && fits) e = cudaStreamSynchronize(q);
+  cudaFree(d_pool);
+  if (fits) {
+    st.bytes_up += lb;
+    st.bytes_down += total;
+  }
+  if (e != cudaSuccess) { ctx->err = std::string("lb2_syms_names: ") + cudaGetErrorString(e); return LB2_E_CUDA; }
+  if (stats) *stats = st;
+  if (!fits) { ctx->err = "lb2_syms_names: the strings exceed pool_cap (*pool_bytes needed)"; return LB2_E_CAPACITY; }
+  return LB2_OK;
+}
+
+}  // extern "C"

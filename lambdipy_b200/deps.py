@@ -4,6 +4,7 @@ shared object the zip's `import`s would load, on the GPU where the zip reader le
 
     python -m lambdipy_b200.deps ZIP [--mount DIR] [--arch x86_64|arm64] [--provided NAME]...
                                      [--max-version GLIBC_2.26]... [--ld-library-path P] [--json]
+                                     [--symbols [--interpreter FILE]... [--runtime-lib DIR]...]
 
 A layer fails at the first `import` when a shared object cannot load: a DT_NEEDED library that neither the zip nor
 the runtime has, a symbol version newer than the runtime's, an object for the other architecture.  The check finds
@@ -30,7 +31,13 @@ that nobody has checked against a Lambda image here; the report names every need
 Deviations from the loader, each documented in DESIGN.md section 9.8: a candidate file is taken when it exists (glibc
 also skips a candidate of the wrong ELF class or machine and searches on; here that is an `arch` problem); the
 executable's own DT_RPATH, ld.so.cache entries beyond `provided`, libraries opened by `dlopen` at run time and the
-effects of import order between roots are not modelled; symbol resolution is checked only as far as version needs."""
+effects of import order between roots are not modelled.
+
+With symbols=True (--symbols) the check also looks up, on the GPU, every symbol that an object's relocations bind when
+`dlopen` loads it with RTLD_NOW, as glibc's do_lookup_x and check_match do, in the scope of the interpreter's global
+objects followed by the root's closure (lb2_syms_*; DESIGN.md section 9.9).  This finds the `undefined symbol` of an
+extension module built against another version of a library the zip carries.  Only counts and the failed lookups come
+back from the device."""
 import json
 import os
 import posixpath
@@ -58,6 +65,7 @@ SYMLINK_HOPS = 40
 BATCH_BYTES = Z.BATCH_BYTES
 _VERSION = re.compile(r"^([A-Za-z][A-Za-z0-9]*)_(\d+(?:\.\d+)*)$")
 VER_FLG_WEAK = 2
+CLASS_IN_ZIP, CLASS_RUNTIME, CLASS_INTERPRETER = 0, 1, 2  # where a reference's definition was found
 
 
 class GpuElfParser:
@@ -116,6 +124,98 @@ class GpuElfParser:
 
     def close(self):
         self._release()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+class GpuSymbolResolver:
+    """lb2_syms_* over objects in device memory, for a whole check: index(refs) copies each object's symbol tables
+    into the resolver's device arena while the object is still there and returns [(id, status, references)];
+    resolve(jobs, scope, classes) looks every reference of jobs' objects up in their scopes and returns ([(in_zip,
+    runtime, interpreter) per job], [(job, reference) found nowhere, sorted]); names(jobs, misses) gives [(name, version,
+    version file)] of misses.  uploaded / downloaded count the bytes that crossed the bus."""
+
+    def __init__(self, ctx):
+        self._ctx, h = ctx, C.c_void_p()
+        ctx.check(ctx.lib.lb2_syms_create(ctx.h, C.byref(h)))
+        self._h = h
+        self.uploaded = self.downloaded = 0
+        self._miss_cap = 1 << 12
+        self._stats = {"index_ms": 0.0, "refs_ms": 0.0, "resolve_ms": 0.0, "references": 0, "lookups": 0}
+
+    def _account(self, st):
+        self.uploaded += st.bytes_up
+        self.downloaded += st.bytes_down
+        for k in ("index_ms", "refs_ms", "resolve_ms"):
+            self._stats[k] += getattr(st, k)
+
+    def index(self, refs):
+        n = len(refs)
+        if not n:
+            return []
+        ptrs = (C.c_uint64 * n)(*[a for a, _ in refs])
+        sizes = (C.c_uint64 * n)(*[k for _, k in refs])
+        ids, objs, st = (C.c_uint32 * n)(), (N.SymObject * n)(), N.SymsStats()
+        rc = self._ctx.lib.lb2_syms_index(self._h, ptrs, sizes, n, ids, objs, C.byref(st))
+        self._account(st)
+        if rc == N.LB2_E_CAPACITY:  # the arena cannot grow by this batch: index it in halves
+            if n == 1:
+                raise Z.DeviceTooSmall("lb2_syms_index: no device memory for the symbol arena")
+            return self.index(refs[:n // 2]) + self.index(refs[n // 2:])
+        self._ctx.check(rc)
+        self._stats["references"] += st.references
+        return [(ids[i], objs[i].status, objs[i].nrefs) for i in range(n)]
+
+    def resolve(self, jobs, scope, classes):
+        nj, ns = len(jobs), len(scope)
+        cj = (N.SymJob * max(nj, 1))(*[N.SymJob(o, off, ln, 0) for o, off, ln in jobs])
+        cs = (C.c_uint32 * max(ns, 1))(*scope)
+        cc = (C.c_uint8 * max(len(classes), 1))(*classes)
+        counts, nm, st = (C.c_uint32 * max(3 * nj, 1))(), C.c_uint32(), N.SymsStats()
+        while True:
+            miss = (N.SymMiss * self._miss_cap)()
+            rc = self._ctx.lib.lb2_syms_resolve(self._h, cj, nj, cs, ns, cc, counts, miss, self._miss_cap, C.byref(nm),
+                                                C.byref(st))
+            self._account(st)
+            if rc == N.LB2_E_CAPACITY:
+                self._miss_cap = max(2 * self._miss_cap, nm.value)
+                continue
+            self._ctx.check(rc)
+            break
+        self._stats["lookups"] += st.lookups
+        return ([tuple(counts[3 * j:3 * j + 3]) for j in range(nj)],
+                sorted((miss[i].job, miss[i].ref) for i in range(nm.value)))  # the kernel appends them in any order
+
+    def names(self, jobs, misses):
+        n = len(misses)
+        if not n:
+            return []
+        cj = (N.SymJob * max(len(jobs), 1))(*[N.SymJob(o, off, ln, 0) for o, off, ln in jobs])
+        cm = (N.SymMiss * n)(*[N.SymMiss(j, r) for j, r in misses])
+        offs, need, st, cap = (C.c_uint64 * n)(), C.c_uint64(), N.SymsStats(), 64 * n
+        while True:
+            pool = C.create_string_buffer(cap)
+            rc = self._ctx.lib.lb2_syms_names(self._h, cj, len(jobs), cm, n, offs, pool, cap, C.byref(need), C.byref(st))
+            self._account(st)
+            if rc == N.LB2_E_CAPACITY:
+                cap = need.value
+                continue
+            self._ctx.check(rc)
+            break
+        raw = pool.raw
+        return [tuple(x.decode("utf-8", "surrogateescape") for x in raw[offs[i]:].split(b"\0", 3)[:3]) for i in range(n)]
+
+    def stats(self):
+        return dict(self._stats)
+
+    def close(self):
+        if self._h:
+            self._ctx.lib.lb2_syms_destroy(self._h)
+            self._h = None
 
     def __enter__(self):
         return self
@@ -319,8 +419,14 @@ class _Model:
 
 
 def check_with(zip_path, decoder, parser, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVIDED,
-               max_versions=None, ld_library_path=LAMBDA_LD_LIBRARY_PATH, batch_bytes=BATCH_BYTES):
-    """check_zip with the engines given (GpuUnzipDecoder and GpuElfParser, or stand-ins with the same interfaces)."""
+               max_versions=None, ld_library_path=LAMBDA_LD_LIBRARY_PATH, batch_bytes=BATCH_BYTES, *, symbols=False,
+               interpreter=(), runtime_libs=(), resolver=None, python_names=True):
+    """check_zip with the engines given (GpuUnzipDecoder, GpuElfParser and, with symbols=True, GpuSymbolResolver, or
+    stand-ins with the same interfaces).  python_names=False turns off the rule that counts an unresolved Py* / _Py*
+    name as the interpreter's when no interpreter is given."""
+    if symbols and resolver is None:
+        raise ValueError("symbols=True needs a resolver")
+    sym_ids = {}
     if arch not in MACHINES:
         raise ValueError("arch=%r: expected one of %s" % (arch, ", ".join(MACHINES)))
     ceilings = {}
@@ -347,6 +453,9 @@ def check_with(zip_path, decoder, parser, mount="/var/task", arch="x86_64", prov
                     raise Z.BadZipMember(zi.filename, {Z.UNZIP_BAD_DATA: "Invalid DEFLATE data", Z.UNZIP_BAD_CRC: "Bad CRC-32",
                                                        Z.UNZIP_WRONG_SIZE: "Wrong uncompressed size"}[status])
                 refs.append(ref if ref is not None else parser.upload(zf.read(zi)))
+            if symbols:  # before parse(), which frees the uploads
+                for (key, zi, _), got in zip(part, resolver.index(refs)):
+                    sym_ids[id(zi)] = got
             for (key, zi, _), (status, machine, records) in zip(part, parser.parse(refs)):
                 objs[id(zi)] = _Obj(zi, status, machine, records)
 
@@ -374,6 +483,9 @@ def check_with(zip_path, decoder, parser, mount="/var/task", arch="x86_64", prov
                            "bytes_up": uploaded + parser.uploaded, "bytes_down": parser.downloaded,
                            "inflate_ms": decoder.stats().get("kernel_ms", 0.0),
                            "parse_ms": parser.stats().get("kernel_ms", 0.0)}
+        if symbols:
+            _Symbols(tree, roots, objs, model, path_of, sym_ids, parser, resolver, provided, interpreter, runtime_libs,
+                     python_names).check(report)
     return report
 
 
@@ -446,8 +558,181 @@ def _report(tree, roots, objs, model, path_of, arch, ceilings):
             "provided_used": {k: sorted(v) for k, v in sorted(provided_used.items())}}
 
 
+class _Symbols:
+    """The symbol check of check_with(symbols=True) over the parsed zip: the scope of each root, the lookups of the
+    references of every object in its closure (by the resolver), and the classes and problems of what is left."""
+
+    def __init__(self, tree, roots, objs, model, path_of, sym_ids, parser, resolver, provided, interpreter,
+                 runtime_libs, python_names):
+        self.tree, self.roots, self.objs, self.model, self.path_of = tree, roots, objs, model, path_of
+        self.sym_ids, self.parser, self.resolver = sym_ids, parser, resolver
+        self.provided, self.interpreter, self.runtime_libs = frozenset(provided), list(interpreter), list(runtime_libs)
+        self.python_names = python_names
+        self.host = {}  # real path of an interpreter file or runtime library -> (class, (id, status, refs), _Obj, path)
+
+    def _load(self, path, cls):
+        real = os.path.realpath(path)
+        if real not in self.host:
+            with open(real, "rb") as f:
+                data = f.read()
+            ref = self.parser.upload(data)
+            sym = self.resolver.index([ref])[0]
+            status, machine, records = self.parser.parse([ref])[0]
+            self.host[real] = (cls, sym, _Obj(None, status, machine, records), path)
+        return real
+
+    def _runtime(self, name):
+        """the real path of `name` in runtime_libs, loaded, or None"""
+        for d in self.runtime_libs:
+            p = os.path.join(d, name)
+            if os.path.isfile(p):
+                return self._load(p, CLASS_RUNTIME)
+        return None
+
+    def _host_needs(self, real):
+        """the nodes of a host object's DT_NEEDED, found in its DT_RPATH / DT_RUNPATH ($ORIGIN expanded), then in
+        runtime_libs; a name found nowhere is a provided node when it is in `provided`, else left out"""
+        cls, _, o, path = self.host[real]
+        dirs = []
+        for rp in (o.rpath, o.runpath):
+            for d in rp.split(":") if rp else ():
+                dirs.append(d.replace("${ORIGIN}", os.path.dirname(path)).replace("$ORIGIN", os.path.dirname(path)))
+        out = []
+        for name in o.needed:
+            node = next((("host", self._load(os.path.join(d, name), cls)) for d in dirs
+                         if os.path.isfile(os.path.join(d, name))), None)
+            if node is None:
+                r = self._runtime(name)
+                node = ("host", r) if r else ("provided", name) if name in self.provided else None
+            if node is not None:
+                out.append(node)
+        return out
+
+    def _bfs(self, order, needs):
+        seen, q = set(order), 0
+        while q < len(order):
+            for node in needs(order[q]):
+                if node not in seen:
+                    seen.add(node)
+                    order.append(node)
+            q += 1
+        return order
+
+    def _local(self, root_zi, resolutions):
+        """the root's search list: the closure's breadth-first order with the provided libraries at their places"""
+        by_loader = {}
+        for _, lzi, name, how, found in resolutions:
+            by_loader.setdefault(id(lzi), []).append((name, how, found))
+
+        def needs(node):
+            kind, key = node
+            if kind == "host":
+                return self._host_needs(key)
+            out = []
+            for name, how, found in by_loader.get(key, []) if kind == "zip" else ():
+                if how == "provided":
+                    r = self._runtime(name)
+                    out.append(("host", r) if r else ("provided", name))
+                elif how != "missing":
+                    out.append(("zip", id(self.tree.lookup(found))))
+            return out
+        return self._bfs([("zip", id(root_zi))], needs)
+
+    def check(self, report):
+        up0, down0 = self.parser.uploaded, self.parser.downloaded
+        problems, notes = report["problems"], report["notes"]
+        seen = {(p["object"], p["kind"], p["detail"]) for p in problems + notes}
+
+        def problem(obj, kind, detail, weak=False):
+            if (obj, kind, detail) not in seen:
+                seen.add((obj, kind, detail))
+                (notes if weak else problems).append({"object": obj, "kind": kind, "detail": detail})
+
+        glob = self._bfs([("host", self._load(f, CLASS_INTERPRETER)) for f in self.interpreter],
+                         lambda node: self._host_needs(node[1]) if node[0] == "host" else [])
+        jobs, flat, scopes, meta, first, symbols, skipped = [], [], {}, [], {}, {}, 0
+        for root_path, root_zi in self.roots:
+            loaded, resolutions, _ = self.model.closure(root_path, root_zi)
+            if any(r[3] == "missing" for r in resolutions) or any(self.objs[id(zi)].status != N.ELF_OK for _, zi in loaded):
+                skipped += 1
+                continue
+            order, ids, opaque = [], [], []
+            for node in glob + self._local(root_zi, resolutions):
+                if node in order:
+                    continue
+                order.append(node)
+                kind, key = node
+                if kind == "provided":
+                    opaque.append(key)
+                else:
+                    ids.append(self.sym_ids[key][0] if kind == "zip" else self.host[key][1][0])
+            skey = (tuple(ids), tuple(opaque))
+            if skey not in scopes:
+                scopes[skey] = len(flat)
+                flat += ids
+            root = posixpath.normpath(root_path)
+            for p, zi in loaded:
+                p = posixpath.normpath(p)
+                rid, status, nrefs = self.sym_ids[id(zi)]
+                if status != N.SYM_OK:
+                    problem(p, "symbol", "symbol tables %s: not checked" % STATUS_NAMES.get(status, status),
+                            status == N.SYM_UNSUPPORTED)
+                    continue
+                symbols.setdefault(p, {"references": nrefs, "in_zip": 0, "runtime": 0, "trusted": 0, "interpreter": 0,
+                                       "unverified": 0})
+                if nrefs and (rid, skey) not in first:
+                    first[(rid, skey)] = len(jobs)
+                    jobs.append((rid, scopes[skey], len(ids)))
+                    meta.append((p, root, opaque))
+        n_ids = 1 + max([s[0] for s in self.sym_ids.values()] + [h[1][0] for h in self.host.values()] + [0])
+        classes = [CLASS_IN_ZIP] * n_ids
+        for cls, sym, _, _ in self.host.values():
+            classes[sym[0]] = cls
+        counts, misses = self.resolver.resolve(jobs, flat, classes)
+        per = [{"in_zip": c[0], "runtime": c[1], "interpreter": c[2], "trusted": 0, "unverified": 0} for c in counts]
+        reported = set()  # (object, symbol): one problem or note each, under the first root that met it
+        for (j, _), (name, ver, file) in zip(misses, self.resolver.names(jobs, misses)):
+            p, root, opaque = meta[j]
+            label = name + ("@" + ver if ver else "")
+            first_report = (p, label) not in reported
+            reported.add((p, label))
+            if not self.interpreter and self.python_names and name.startswith(("Py", "_Py")):
+                per[j]["interpreter"] += 1
+            elif ver and file in self.provided and self._runtime(file) is None:
+                per[j]["trusted"] += 1
+            elif not ver and opaque:  # glibc binds it to a definition at versym index 2 too (DESIGN.md section 9.9)
+                per[j]["unverified"] += 1
+                if first_report:
+                    problem(p, "symbol", "%s: not found; unverified: %s may define it" % (label, ", ".join(opaque)), True)
+            elif first_report:
+                problem(p, "symbol", "%s: no definition in the load scope of %s" % (label, root))
+        seen_obj = set()
+        for j, (p, _, _) in enumerate(meta):
+            if p not in seen_obj:
+                seen_obj.add(p)
+                symbols[p].update(per[j])
+        # a version need on a provided library read from runtime_libs: its Verdefs must have it
+        for zid, o in self.objs.items():
+            if o.status != N.ELF_OK:
+                continue
+            for f, v, weak in o.verneed:
+                real = self._runtime(f) if f in self.provided else None
+                if real is not None and self.host[real][2].status == N.ELF_OK and v not in self.host[real][2].verdef:
+                    problem(posixpath.normpath(self.path_of[zid]), "version", "%s not defined by %s" % (v, f), weak)
+        st, rs = report["stats"], self.resolver.stats()
+        refs_of = {i: n for i, _, n in self.sym_ids.values()}
+        report["symbols"] = dict(sorted(symbols.items()))
+        st["bytes_up"] += self.parser.uploaded - up0 + self.resolver.uploaded
+        st["bytes_down"] += self.parser.downloaded - down0 + self.resolver.downloaded
+        st.update({"symbols_ms": rs["index_ms"] + rs["refs_ms"] + rs["resolve_ms"], "symbols_index_ms": rs["index_ms"],
+                   "symbols_refs_ms": rs["refs_ms"], "symbols_resolve_ms": rs["resolve_ms"],
+                   "references": sum(refs_of[j[0]] for j in jobs), "lookups": rs["lookups"],
+                   "symbols_skipped": skipped})
+
+
 def check_zip(zip_path, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVIDED, max_versions=None,
-              ld_library_path=LAMBDA_LD_LIBRARY_PATH, ctx=None, batch_bytes=BATCH_BYTES):
+              ld_library_path=LAMBDA_LD_LIBRARY_PATH, ctx=None, batch_bytes=BATCH_BYTES, *, symbols=False,
+              interpreter=(), runtime_libs=()):
     """Check that the shared objects of `zip_path`, unpacked at `mount`, will load on Lambda (see the module docstring
     for the search it restates).  Returns a plain dict:
 
@@ -465,6 +750,17 @@ def check_zip(zip_path, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVI
       libraries; provided_used: {soname: the objects whose need the `provided` list satisfied};
     * stats: members, roots, objects (parsed), rounds, bytes_up, bytes_down, inflate_ms and parse_ms (CUDA events).
 
+    symbols=True also checks that every symbol the objects' relocations look up has a definition in the scope of a
+    `dlopen(root, RTLD_NOW | RTLD_LOCAL)` from the interpreter (DESIGN.md section 9.9): the exported definitions of
+    the `interpreter` files (such as sys.executable) and their DT_NEEDED closure, then the root's closure in load
+    order.  `runtime_libs` are host directories holding the `provided` libraries; one found there takes its place in
+    the scope with its own definitions.  The report gains problems of kind "symbol" (NAME[@VERSION]: no definition in
+    the load scope of ROOT), notes of kind "symbol" (an unversioned name that only a provided library not read could
+    define), "version" problems against the Verdefs of the runtime_libs copies, symbols {object: {references, in_zip,
+    runtime, trusted, interpreter, unverified}} under the first root that checked it, and stats symbols_ms (index,
+    refs and resolve kernels, CUDA events; also split as symbols_index_ms, symbols_refs_ms, symbols_resolve_ms),
+    references, lookups and symbols_skipped (roots with a missing need or an unloadable object, not checked).
+
     Members are inflated by the GPU zip reader and parsed on the GPU (lb2_elf_deps) where they lie; only the records
     and their strings come back.  There is no CPU path: without a GPU this raises."""
     from .tarball import _default_context
@@ -473,7 +769,12 @@ def check_zip(zip_path, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVI
         ctx, own = _default_context()
     try:
         with Z.GpuUnzipDecoder(ctx) as dec, GpuElfParser(ctx) as parser:
-            return check_with(zip_path, dec, parser, mount, arch, provided, max_versions, ld_library_path, batch_bytes)
+            if not symbols:
+                return check_with(zip_path, dec, parser, mount, arch, provided, max_versions, ld_library_path, batch_bytes)
+            with GpuSymbolResolver(ctx) as resolver:
+                return check_with(zip_path, dec, parser, mount, arch, provided, max_versions, ld_library_path,
+                                  batch_bytes, symbols=True, interpreter=interpreter, runtime_libs=runtime_libs,
+                                  resolver=resolver)
     finally:
         if own:
             ctx.close()
@@ -487,6 +788,9 @@ def summary(report):
         lines.append("highest versions needed: " + ", ".join("%s_%s" % kv for kv in report["max_versions"].items()))
     if report["provided_used"]:
         lines.append("satisfied by the runtime list: " + ", ".join(report["provided_used"]))
+    if "symbols" in report:
+        lines.append("symbols: %d references, %d lookups, %d root(s) not checked"
+                     % (st["references"], st["lookups"], st["symbols_skipped"]))
     for p in report["problems"]:
         lines.append("problem: %s: %s: %s" % (p["object"], p["kind"], p["detail"]))
     for p in report["notes"]:
@@ -514,13 +818,20 @@ def main(argv=None, check=check_zip):
     ap.add_argument("--max-version", action="append", default=[], metavar="PREFIX_VERSION",
                     help="the runtime's highest version of a prefix, such as GLIBC_2.26 (repeatable)")
     ap.add_argument("--ld-library-path", default=LAMBDA_LD_LIBRARY_PATH)
+    ap.add_argument("--symbols", action="store_true", help="also check the symbols each object binds when it loads")
+    ap.add_argument("--interpreter", action="append", default=[], metavar="FILE",
+                    help="with --symbols: an ELF file heading the global scope, such as the python executable (repeatable)")
+    ap.add_argument("--runtime-lib", action="append", default=[], metavar="DIR",
+                    help="with --symbols: a directory holding the runtime's provided libraries (repeatable)")
     ap.add_argument("--json", action="store_true", help="print the whole report as JSON")
     args = ap.parse_args(argv)
     try:
         ceilings = dict(_ceiling(t) for t in args.max_version)
         report = check(args.zip, mount=args.mount, arch=args.arch,
                        provided=DEFAULT_PROVIDED if args.provided is None else frozenset(args.provided),
-                       max_versions=ceilings, ld_library_path=args.ld_library_path)
+                       max_versions=ceilings, ld_library_path=args.ld_library_path,
+                       **({"symbols": True, "interpreter": args.interpreter, "runtime_libs": args.runtime_lib}
+                          if args.symbols else {}))
     except (OSError, ValueError, zipfile.BadZipFile) as e:
         print("error: %s" % e, file=sys.stderr)
         return 2
