@@ -37,7 +37,11 @@ With symbols=True (--symbols) the check also looks up, on the GPU, every symbol 
 `dlopen` loads it with RTLD_NOW, as glibc's do_lookup_x and check_match do, in the scope of the interpreter's global
 objects followed by the root's closure (lb2_syms_*; DESIGN.md section 9.9).  This finds the `undefined symbol` of an
 extension module built against another version of a library the zip carries.  Only counts and the failed lookups come
-back from the device."""
+back from the device.
+
+The check runs over entries (check_entries): check_with builds them from a zip's central directory, and the layer
+writers (layer.zip_build / zip_tarballs with check=...) from the entries of the zip they are about to write, with the
+bytes they already hold on the device (DESIGN.md section 9.10)."""
 import json
 import os
 import posixpath
@@ -236,7 +240,7 @@ def decode(objs, recs, pool):
 
 
 class _Obj:
-    """what the loader model needs of one parsed member"""
+    """what the loader model needs of one parsed member (member: its entry's name)"""
 
     def __init__(self, member, status, machine, records):
         self.member, self.status, self.machine = member, status, machine
@@ -263,18 +267,20 @@ class _Obj:
 
 
 class _Tree:
-    """The zip as the file system under `mount`: {absolute path: ZipInfo of a regular file | link target}, and the
-    directories its paths imply."""
+    """The zip as the file system under `mount`: {absolute path: key of a regular file | link target}, and the
+    directories its paths imply.  entries [(key, name, link)]: an opaque key, the entry's name (a directory's ends in
+    "/") and a symlink's target (None for a regular file or a directory)."""
 
-    def __init__(self, zf, mount):
+    def __init__(self, entries, mount):
         self.mount = posixpath.normpath("/" + mount.strip("/")) if mount.strip("/") else "/"
-        self.files, self.links, self.dirs = {}, {}, {self.mount}
+        self.files, self.links, self.dirs, self.names = {}, {}, {self.mount}, {}
         d = self.mount
         while d != "/":
             d = posixpath.dirname(d)
             self.dirs.add(d)
-        for zi in zf.infolist():  # a repeated name: the last entry, as getinfo and extractall leave it
-            name = zi.filename.rstrip("/")
+        for key, entry_name, link in entries:  # a repeated name: the last entry, as getinfo and extractall leave it
+            self.names[key] = entry_name
+            name = entry_name.rstrip("/")
             if not name:
                 continue
             path = posixpath.normpath(posixpath.join(self.mount, name))
@@ -284,15 +290,15 @@ class _Tree:
                 d = posixpath.dirname(d)
             self.files.pop(path, None)
             self.links.pop(path, None)
-            if zi.is_dir():
+            if entry_name.endswith("/"):
                 self.dirs.add(path)
-            elif (zi.external_attr >> 16) & 0o170000 == stat.S_IFLNK:
-                self.links[path] = zf.read(zi).decode("utf-8", "surrogateescape")
+            elif link is not None:
+                self.links[path] = link
             else:
-                self.files[path] = zi
+                self.files[path] = key
 
     def lookup(self, path):
-        """the ZipInfo of the regular file `path` ends at, symlinks followed, or None"""
+        """the key of the regular file `path` ends at, symlinks followed, or None"""
         parts, i, cur, hops = [x for x in path.split("/") if x], 0, [], SYMLINK_HOPS
         while i < len(parts):
             comp = parts[i]
@@ -346,16 +352,16 @@ class _Model:
         self.env = _expand(ld_library_path or "", LAMBDA_TASK_ROOT, arch) if ld_library_path else []
 
     def _find(self, name, obj_path, chain):
-        """(how, path or None, ZipInfo or None) for NEEDED `name` of the object at obj_path loaded through `chain`"""
+        """(how, path or None, key or None) for NEEDED `name` of the object at obj_path loaded through `chain`"""
         if "/" in name:
             path = posixpath.join(LAMBDA_TASK_ROOT, name)
-            zi = self.tree.lookup(path)
-            return ("path", path, zi) if zi is not None else ("missing", None, None)
-        obj = self.objs[id(chain[-1][1])]
+            key = self.tree.lookup(path)
+            return ("path", path, key) if key is not None else ("missing", None, None)
+        obj = self.objs[chain[-1][1]]
         searches = []
         if obj.runpath is None:
-            for p, zi in reversed(chain):
-                o = self.objs[id(zi)]
+            for p, key in reversed(chain):
+                o = self.objs[key]
                 if o.rpath is not None:
                     searches.append(("rpath", _expand(o.rpath, posixpath.dirname(p), self.arch)))
         searches.append(("ld_library_path", self.env))
@@ -366,56 +372,171 @@ class _Model:
                 if name in self.provided and posixpath.normpath(d) in RUNTIME_DIRS:
                     return "provided", None, None
                 path = posixpath.join(d, name)
-                zi = self.tree.lookup(path)
-                if zi is not None:
-                    return how, path, zi
+                key = self.tree.lookup(path)
+                if key is not None:
+                    return how, path, key
         return ("provided", None, None) if name in self.provided else ("missing", None, None)
 
-    def closure(self, root_path, root_zi):
-        """(loaded [(path, ZipInfo)] in load order, [(loader path, its ZipInfo, name, how, path)], unparsed ZipInfos
-        reached)"""
-        loaded = [(root_path, root_zi)]
-        names = {id(root_zi): {root_path}}
-        loader = {id(root_zi): None}
+    def closure(self, root_path, root_key):
+        """(loaded [(path, key)] in load order, [(loader path, its key, name, how, path)], unparsed keys reached)"""
+        loaded = [(root_path, root_key)]
+        names = {root_key: {root_path}}
+        loader = {root_key: None}
         provided_loaded = set()
         resolutions, pending = [], []
         q = 0
         while q < len(loaded):
-            path, zi = loaded[q]
+            path, key = loaded[q]
             q += 1
-            obj = self.objs.get(id(zi))
+            obj = self.objs.get(key)
             if obj is None:
-                pending.append(zi)
+                pending.append(key)
                 continue
             if obj.status != N.ELF_OK:
                 continue
-            chain, z = [], zi  # this object, its loader, and on up to the root
+            chain, z = [], key  # this object, its loader, and on up to the root
             while z is not None:
-                chain.insert(0, (next(p for p, y in loaded if y is z), z))
-                z = loader[id(z)]
+                chain.insert(0, (next(p for p, y in loaded if y == z), z))
+                z = loader[z]
             for name in obj.needed:
-                hit = next((y for p, y in loaded if name in names[id(y)] or
-                            (id(y) in self.objs and self.objs[id(y)].soname == name)), None)
+                hit = next((y for p, y in loaded if name in names[y] or
+                            (y in self.objs and self.objs[y].soname == name)), None)
                 if hit is not None:
-                    resolutions.append((path, zi, name, "loaded", next(p for p, y in loaded if y is hit)))
-                    names[id(hit)].add(name)
+                    resolutions.append((path, key, name, "loaded", next(p for p, y in loaded if y == hit)))
+                    names[hit].add(name)
                     continue
                 if name in provided_loaded:
-                    resolutions.append((path, zi, name, "provided", None))
+                    resolutions.append((path, key, name, "provided", None))
                     continue
-                how, found, fzi = self._find(name, path, chain)
-                if fzi is not None and id(fzi) in names:  # the same file by another name: one object
-                    names[id(fzi)].add(name)
-                    resolutions.append((path, zi, name, how, next(p for p, y in loaded if y is fzi)))
+                how, found, fkey = self._find(name, path, chain)
+                if fkey is not None and fkey in names:  # the same file by another name: one object
+                    names[fkey].add(name)
+                    resolutions.append((path, key, name, how, next(p for p, y in loaded if y == fkey)))
                     continue
-                resolutions.append((path, zi, name, how, found))
+                resolutions.append((path, key, name, how, found))
                 if how == "provided":
                     provided_loaded.add(name)
-                elif fzi is not None:
-                    loaded.append((found, fzi))
-                    names[id(fzi)] = {name, found}
-                    loader[id(fzi)] = zi
+                elif fkey is not None:
+                    loaded.append((found, fkey))
+                    names[fkey] = {name, found}
+                    loader[fkey] = key
         return loaded, resolutions, pending
+
+
+CHECK_KEYS = ("mount", "arch", "provided", "max_versions", "ld_library_path", "symbols", "interpreter", "runtime_libs")
+
+
+class CheckFailed(Exception):
+    """A layer writer's check found problems: report is what check_zip would return for the zip it did not write."""
+
+    def __init__(self, report):
+        first = report["problems"][0]
+        super().__init__("%d problem(s), the first: %s: %s: %s" % (len(report["problems"]), first["object"],
+                                                                   first["kind"], first["detail"]))
+        self.report = report
+
+
+def _ceilings(arch, max_versions):
+    """{prefix: version key} of max_versions; ValueError for an unknown arch or a version that is not dotted"""
+    if arch not in MACHINES:
+        raise ValueError("arch=%r: expected one of %s" % (arch, ", ".join(MACHINES)))
+    ceilings = {}
+    for prefix, v in (max_versions or {}).items():
+        if not re.fullmatch(r"\d+(?:\.\d+)*", str(v)):
+            raise ValueError("max_versions[%r]=%r: expected a dotted version such as 2.26" % (prefix, v))
+        ceilings[prefix] = _version_key(str(v))
+    return ceilings
+
+
+def check_options(check):
+    """check_zip's keyword arguments in the dict `check`, refused as check_with refuses them: ValueError for a key that
+    is not one of CHECK_KEYS, an unknown arch or a max_versions value that is not a dotted version"""
+    if not isinstance(check, dict):
+        raise ValueError("check=%r: expected a dict of check_zip's keyword arguments" % (check,))
+    unknown = sorted(set(check) - set(CHECK_KEYS))
+    if unknown:
+        raise ValueError("check: unknown key(s) %s; expected some of %s" % (", ".join(map(repr, unknown)),
+                                                                         ", ".join(CHECK_KEYS)))
+    _ceilings(check.get("arch", "x86_64"), check.get("max_versions"))
+    return dict(check)
+
+
+def member_decoder(decoder, parser, members, batch_bytes=BATCH_BYTES):
+    """The decode step of check_entries over zip members, members {key: (ZipInfo, (ZipFile, its open file, its size))}:
+    a round's members go to the GPU reader in batches of about batch_bytes (Z.decode_members, halved on a device too
+    small); a member the reader does not take is read by the stdlib and uploaded through the parser."""
+    def decode(keys, consume):
+        def part_done(part, decoded, whole):
+            refs = []
+            for key, zi, (zf, _, _) in part:
+                status, ref = decoded.get(key, (Z.UNZIP_OK, None))
+                if status != Z.UNZIP_OK:
+                    raise Z.BadZipMember(zi.filename, {Z.UNZIP_BAD_DATA: "Invalid DEFLATE data", Z.UNZIP_BAD_CRC: "Bad CRC-32",
+                                                       Z.UNZIP_WRONG_SIZE: "Wrong uncompressed size"}[status])
+                refs.append(ref if ref is not None else parser.upload(zf.read(zi)))
+            consume([key for key, _, _ in part], refs)
+
+        uploaded, batch, cost = 0, [], 0
+        for key in keys:
+            zi, source = members[key]
+            c = zi.compress_size + 3 * zi.file_size + 1024
+            if batch and cost + c > batch_bytes:
+                uploaded += Z.decode_members(decoder, batch, part_done)
+                batch, cost = [], 0
+            batch.append((key, zi, source))
+            cost += c
+        if batch:
+            uploaded += Z.decode_members(decoder, batch, part_done)
+        return uploaded
+    return decode
+
+
+def check_entries(entries, decode, parser, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVIDED,
+                  max_versions=None, ld_library_path=LAMBDA_LD_LIBRARY_PATH, *, symbols=False, interpreter=(),
+                  runtime_libs=(), resolver=None, python_names=True):
+    """The check over the entries of a zip: entries [(key, name, link)] (an opaque hashable key, the entry's name, a
+    symlink's target or None), in the zip's order.  decode(keys, consume) puts the regular files of a round on the
+    device: it calls consume(part, refs) once or more, part a list of the keys and refs their (device address, size),
+    valid until consume returns, and returns the bytes it uploaded.  The report has no inflate_ms: the caller knows
+    what its decode step cost."""
+    if symbols and resolver is None:
+        raise ValueError("symbols=True needs a resolver")
+    ceilings = _ceilings(arch, max_versions)
+    sym_ids = {}
+    tree = _Tree(entries, mount)
+    path_of = {}
+    for p, key in tree.files.items():
+        path_of.setdefault(key, p)
+    roots = [(p, key) for p, key in sorted(tree.files.items())
+             if tree.names[key].rsplit("/", 1)[-1].endswith(Z.SO_SUFFIX)]  # Z.selected_for_strip of a regular file
+    objs, rounds, uploaded = {}, 0, 0
+    model = _Model(tree, objs, arch, provided, ld_library_path)
+
+    def consume(keys, refs):
+        if symbols:  # before parse(), which frees the uploads
+            for key, got in zip(keys, resolver.index(refs)):
+                sym_ids[key] = got
+        for key, (status, machine, records) in zip(keys, parser.parse(refs)):
+            objs[key] = _Obj(tree.names[key], status, machine, records)
+
+    todo = [key for _, key in roots]
+    while todo:
+        rounds += 1
+        uploaded += decode(todo, consume)
+        seen, todo = set(), []
+        for p, key in roots:
+            for k in model.closure(p, key)[2]:
+                if k not in objs and k not in seen:
+                    seen.add(k)
+                    todo.append(k)
+    report = _report(tree, roots, objs, model, path_of, arch, ceilings)
+    report["stats"] = {"members": len(entries), "roots": len(roots), "objects": len(objs), "rounds": rounds,
+                       "bytes_up": uploaded + parser.uploaded, "bytes_down": parser.downloaded,
+                       "parse_ms": parser.stats().get("kernel_ms", 0.0)}
+    if symbols:
+        _Symbols(tree, roots, objs, model, path_of, sym_ids, parser, resolver, provided, interpreter, runtime_libs,
+                 python_names).check(report)
+    return report
 
 
 def check_with(zip_path, decoder, parser, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVIDED,
@@ -426,66 +547,19 @@ def check_with(zip_path, decoder, parser, mount="/var/task", arch="x86_64", prov
     name as the interpreter's when no interpreter is given."""
     if symbols and resolver is None:
         raise ValueError("symbols=True needs a resolver")
-    sym_ids = {}
-    if arch not in MACHINES:
-        raise ValueError("arch=%r: expected one of %s" % (arch, ", ".join(MACHINES)))
-    ceilings = {}
-    for prefix, v in (max_versions or {}).items():
-        if not re.fullmatch(r"\d+(?:\.\d+)*", str(v)):
-            raise ValueError("max_versions[%r]=%r: expected a dotted version such as 2.26" % (prefix, v))
-        ceilings[prefix] = _version_key(str(v))
+    _ceilings(arch, max_versions)
     with zipfile.ZipFile(zip_path) as zf, open(zip_path, "rb") as src:
         src.seek(0, os.SEEK_END)
         source = (zf, src, src.tell())
-        tree = _Tree(zf, mount)
-        path_of = {}
-        for p, zi in tree.files.items():
-            path_of.setdefault(id(zi), p)
-        roots = [(p, zi) for p, zi in sorted(tree.files.items()) if Z.selected_for_strip(zi)]
-        objs, rounds, uploaded = {}, 0, 0
-        model = _Model(tree, objs, arch, provided, ld_library_path)
-
-        def consume(part, decoded, whole):
-            refs = []
-            for key, zi, _ in part:
-                status, ref = decoded.get(key, (Z.UNZIP_OK, None))
-                if status != Z.UNZIP_OK:
-                    raise Z.BadZipMember(zi.filename, {Z.UNZIP_BAD_DATA: "Invalid DEFLATE data", Z.UNZIP_BAD_CRC: "Bad CRC-32",
-                                                       Z.UNZIP_WRONG_SIZE: "Wrong uncompressed size"}[status])
-                refs.append(ref if ref is not None else parser.upload(zf.read(zi)))
-            if symbols:  # before parse(), which frees the uploads
-                for (key, zi, _), got in zip(part, resolver.index(refs)):
-                    sym_ids[id(zi)] = got
-            for (key, zi, _), (status, machine, records) in zip(part, parser.parse(refs)):
-                objs[id(zi)] = _Obj(zi, status, machine, records)
-
-        todo = [zi for _, zi in roots]
-        while todo:
-            rounds += 1
-            batch, cost = [], 0
-            for zi in todo:
-                c = zi.compress_size + 3 * zi.file_size + 1024
-                if batch and cost + c > batch_bytes:
-                    uploaded += Z.decode_members(decoder, batch, consume)
-                    batch, cost = [], 0
-                batch.append((id(zi), zi, source))
-                cost += c
-            if batch:
-                uploaded += Z.decode_members(decoder, batch, consume)
-            seen, todo = set(), []
-            for p, zi in roots:
-                for z in model.closure(p, zi)[2]:
-                    if id(z) not in objs and id(z) not in seen:
-                        seen.add(id(z))
-                        todo.append(z)
-        report = _report(tree, roots, objs, model, path_of, arch, ceilings)
-        report["stats"] = {"members": len(zf.infolist()), "roots": len(roots), "objects": len(objs), "rounds": rounds,
-                           "bytes_up": uploaded + parser.uploaded, "bytes_down": parser.downloaded,
-                           "inflate_ms": decoder.stats().get("kernel_ms", 0.0),
-                           "parse_ms": parser.stats().get("kernel_ms", 0.0)}
-        if symbols:
-            _Symbols(tree, roots, objs, model, path_of, sym_ids, parser, resolver, provided, interpreter, runtime_libs,
-                     python_names).check(report)
+        infos = zf.infolist()
+        entries = [(i, zi.filename, zf.read(zi).decode("utf-8", "surrogateescape")
+                    if not zi.is_dir() and (zi.external_attr >> 16) & 0o170000 == stat.S_IFLNK else None)
+                   for i, zi in enumerate(infos)]
+        decode = member_decoder(decoder, parser, {i: (zi, source) for i, zi in enumerate(infos)}, batch_bytes)
+        report = check_entries(entries, decode, parser, mount, arch, provided, max_versions, ld_library_path,
+                               symbols=symbols, interpreter=interpreter, runtime_libs=runtime_libs, resolver=resolver,
+                               python_names=python_names)
+    report["stats"]["inflate_ms"] = decoder.stats().get("kernel_ms", 0.0)
     return report
 
 
@@ -500,37 +574,37 @@ def _report(tree, roots, objs, model, path_of, arch, ceilings):
             (notes if weak else problems).append({"object": obj, "kind": kind, "detail": detail})
 
     objects, closures, resolved = {}, {}, {}
-    for zid, o in objs.items():
-        p = path_of[zid]
-        objects[p] = {"member": o.member.filename, "status": STATUS_NAMES.get(o.status, str(o.status)),
+    for key, o in objs.items():
+        p = path_of[key]
+        objects[p] = {"member": o.member, "status": STATUS_NAMES.get(o.status, str(o.status)),
                       "machine": o.machine, "soname": o.soname, "rpath": o.rpath, "runpath": o.runpath, "needed": None,
                       "version_needs": [{"file": f, "version": v, "weak": w} for f, v, w in o.verneed],
                       "version_defs": sorted(o.verdef)}
-    for root_path, root_zi in roots:
-        loaded, resolutions, _ = model.closure(root_path, root_zi)
-        closures[root_path] = [path_of[id(zi)] for _, zi in loaded]
+    for root_path, root_key in roots:
+        loaded, resolutions, _ = model.closure(root_path, root_key)
+        closures[root_path] = [path_of[key] for _, key in loaded]
         by_name, filled = {}, set()  # names in this closure -> (how, path)
-        resolved[root_path] = [{"object": path_of[id(lzi)], "name": name, "how": how,
-                                "path": found and posixpath.normpath(found)} for _, lzi, name, how, found in resolutions]
-        for loader_path, lzi, name, how, found in resolutions:
+        resolved[root_path] = [{"object": path_of[lkey], "name": name, "how": how,
+                                "path": found and posixpath.normpath(found)} for _, lkey, name, how, found in resolutions]
+        for loader_path, lkey, name, how, found in resolutions:
             by_name.setdefault(name, (how, found))
             loader_path = posixpath.normpath(loader_path)
-            o = objects[path_of[id(lzi)]]
+            o = objects[path_of[lkey]]
             if o["needed"] is None:
                 o["needed"] = []
-                filled.add(id(lzi))
-            if id(lzi) in filled:
+                filled.add(lkey)
+            if lkey in filled:
                 o["needed"].append({"name": name, "how": how, "path": found and posixpath.normpath(found)})
             if how == "missing":
                 problem(loader_path, "missing", "%s: not in the zip, the search path or the runtime" % name)
             elif how == "provided":
                 provided_used.setdefault(name, set()).add(loader_path)
         filled = set()
-        for p, zi in loaded:
+        for p, key in loaded:
             p = posixpath.normpath(p)
-            o = objs[id(zi)]
+            o = objs[key]
             if o.status != N.ELF_OK:
-                problem(p, "unloadable", "%s: %s" % (o.member.filename, STATUS_NAMES.get(o.status, o.status)))
+                problem(p, "unloadable", "%s: %s" % (o.member, STATUS_NAMES.get(o.status, o.status)))
                 continue
             if o.machine != MACHINES[arch]:
                 problem(p, "arch", "e_machine %d, not %s (%d)" % (o.machine, arch, MACHINES[arch]))
@@ -546,7 +620,7 @@ def _report(tree, roots, objs, model, path_of, arch, ceilings):
                             problem(p, "version", "%s from %s is newer than the runtime's %s_%s"
                                     % (v, f, prefix, ".".join(map(str, ceilings[prefix]))), weak)
                 elif found is not None:
-                    t = objs.get(id(tree.lookup(found)))
+                    t = objs.get(tree.lookup(found))
                     if t is not None and t.status == N.ELF_OK and v not in t.verdef:
                         if not t.verdef:
                             problem(p, "version", "%s: %s has no version information" % (v, f), True)
@@ -618,11 +692,11 @@ class _Symbols:
             q += 1
         return order
 
-    def _local(self, root_zi, resolutions):
+    def _local(self, root_key, resolutions):
         """the root's search list: the closure's breadth-first order with the provided libraries at their places"""
         by_loader = {}
-        for _, lzi, name, how, found in resolutions:
-            by_loader.setdefault(id(lzi), []).append((name, how, found))
+        for _, lkey, name, how, found in resolutions:
+            by_loader.setdefault(lkey, []).append((name, how, found))
 
         def needs(node):
             kind, key = node
@@ -634,9 +708,9 @@ class _Symbols:
                     r = self._runtime(name)
                     out.append(("host", r) if r else ("provided", name))
                 elif how != "missing":
-                    out.append(("zip", id(self.tree.lookup(found))))
+                    out.append(("zip", self.tree.lookup(found)))
             return out
-        return self._bfs([("zip", id(root_zi))], needs)
+        return self._bfs([("zip", root_key)], needs)
 
     def check(self, report):
         up0, down0 = self.parser.uploaded, self.parser.downloaded
@@ -651,13 +725,13 @@ class _Symbols:
         glob = self._bfs([("host", self._load(f, CLASS_INTERPRETER)) for f in self.interpreter],
                          lambda node: self._host_needs(node[1]) if node[0] == "host" else [])
         jobs, flat, scopes, meta, first, symbols, skipped = [], [], {}, [], {}, {}, 0
-        for root_path, root_zi in self.roots:
-            loaded, resolutions, _ = self.model.closure(root_path, root_zi)
-            if any(r[3] == "missing" for r in resolutions) or any(self.objs[id(zi)].status != N.ELF_OK for _, zi in loaded):
+        for root_path, root_key in self.roots:
+            loaded, resolutions, _ = self.model.closure(root_path, root_key)
+            if any(r[3] == "missing" for r in resolutions) or any(self.objs[k].status != N.ELF_OK for _, k in loaded):
                 skipped += 1
                 continue
             order, ids, opaque = [], [], []
-            for node in glob + self._local(root_zi, resolutions):
+            for node in glob + self._local(root_key, resolutions):
                 if node in order:
                     continue
                 order.append(node)
@@ -671,9 +745,9 @@ class _Symbols:
                 scopes[skey] = len(flat)
                 flat += ids
             root = posixpath.normpath(root_path)
-            for p, zi in loaded:
+            for p, key in loaded:
                 p = posixpath.normpath(p)
-                rid, status, nrefs = self.sym_ids[id(zi)]
+                rid, status, nrefs = self.sym_ids[key]
                 if status != N.SYM_OK:
                     problem(p, "symbol", "symbol tables %s: not checked" % STATUS_NAMES.get(status, status),
                             status == N.SYM_UNSUPPORTED)
@@ -712,13 +786,13 @@ class _Symbols:
                 seen_obj.add(p)
                 symbols[p].update(per[j])
         # a version need on a provided library read from runtime_libs: its Verdefs must have it
-        for zid, o in self.objs.items():
+        for key, o in self.objs.items():
             if o.status != N.ELF_OK:
                 continue
             for f, v, weak in o.verneed:
                 real = self._runtime(f) if f in self.provided else None
                 if real is not None and self.host[real][2].status == N.ELF_OK and v not in self.host[real][2].verdef:
-                    problem(posixpath.normpath(self.path_of[zid]), "version", "%s not defined by %s" % (v, f), weak)
+                    problem(posixpath.normpath(self.path_of[key]), "version", "%s not defined by %s" % (v, f), weak)
         st, rs = report["stats"], self.resolver.stats()
         refs_of = {i: n for i, _, n in self.sym_ids.values()}
         report["symbols"] = dict(sorted(symbols.items()))
@@ -805,12 +879,8 @@ def _ceiling(text):
     return m.group(1), m.group(2)
 
 
-def main(argv=None, check=check_zip):
-    """exit status 0: no problem; 1: problems; 2: a refused input or a usage error"""
-    import argparse
-    ap = argparse.ArgumentParser(prog="python -m lambdipy_b200.deps",
-                                 description="check that the shared objects of a Lambda zip will load there")
-    ap.add_argument("zip")
+def add_check_arguments(ap):
+    """the check's options on the ArgumentParser ap; returns their destinations (check_kwargs reads them)"""
     ap.add_argument("--mount", default="/var/task", help="where the zip is unpacked: /var/task (function) or /opt (layer)")
     ap.add_argument("--arch", choices=sorted(MACHINES), default="x86_64")
     ap.add_argument("--provided", action="append", metavar="NAME",
@@ -823,15 +893,30 @@ def main(argv=None, check=check_zip):
                     help="with --symbols: an ELF file heading the global scope, such as the python executable (repeatable)")
     ap.add_argument("--runtime-lib", action="append", default=[], metavar="DIR",
                     help="with --symbols: a directory holding the runtime's provided libraries (repeatable)")
+    return ("mount", "arch", "provided", "max_version", "ld_library_path", "symbols", "interpreter", "runtime_lib")
+
+
+def check_kwargs(args):
+    """check_zip's keyword arguments from the options add_check_arguments defined; ValueError for a --max-version
+    that is not PREFIX_VERSION"""
+    return dict(mount=args.mount, arch=args.arch,
+                provided=DEFAULT_PROVIDED if args.provided is None else frozenset(args.provided),
+                max_versions=dict(_ceiling(t) for t in args.max_version), ld_library_path=args.ld_library_path,
+                **({"symbols": True, "interpreter": args.interpreter, "runtime_libs": args.runtime_lib}
+                   if args.symbols else {}))
+
+
+def main(argv=None, check=check_zip):
+    """exit status 0: no problem; 1: problems; 2: a refused input or a usage error"""
+    import argparse
+    ap = argparse.ArgumentParser(prog="python -m lambdipy_b200.deps",
+                                 description="check that the shared objects of a Lambda zip will load there")
+    ap.add_argument("zip")
+    add_check_arguments(ap)
     ap.add_argument("--json", action="store_true", help="print the whole report as JSON")
     args = ap.parse_args(argv)
     try:
-        ceilings = dict(_ceiling(t) for t in args.max_version)
-        report = check(args.zip, mount=args.mount, arch=args.arch,
-                       provided=DEFAULT_PROVIDED if args.provided is None else frozenset(args.provided),
-                       max_versions=ceilings, ld_library_path=args.ld_library_path,
-                       **({"symbols": True, "interpreter": args.interpreter, "runtime_libs": args.runtime_lib}
-                          if args.symbols else {}))
+        report = check(args.zip, **check_kwargs(args))
     except (OSError, ValueError, zipfile.BadZipFile) as e:
         print("error: %s" % e, file=sys.stderr)
         return 2

@@ -26,7 +26,11 @@ wheel member's DEFLATE body is copied into the zip as it is.
 
     zip_build(dst, tarballs=(), wheels=(), prefix="", keep_tests=())
     python -m lambdipy_b200.layer DST [SRC ...] --wheel WHL [--wheel WHL ...] [--keep-tests NAME] [--clean]
+
+Both writers take check={...} (--check): deps.check_zip's check of the zip, run on the stripped objects where they lie
+on the device before the zip is written; a problem raises deps.CheckFailed and writes nothing (DESIGN.md section 9.10).
 """
+import contextlib
 import ctypes as C
 import email.parser
 import importlib.metadata
@@ -42,6 +46,7 @@ import zipfile
 import zlib
 
 from . import _native as N
+from . import deps as D
 from . import seek_table as ST
 from . import tarball as T
 from . import zipfile_gpu as Z
@@ -233,12 +238,14 @@ def zip_info(path, node, size, umask):
 
 
 def zip_with(srcs, dst, reader, indexer, stripper, encoder, prefix="", fallback_host_strip=True,
-             tolerate_non_elf=False):
+             tolerate_non_elf=False, check=None, parser=None, resolver=None):
     """zip_tarballs with the engines given (tarball.GpuTarReader, tarball.GpuTarIndex, zipfile_gpu.GpuStripper,
-    zipfile_gpu.GpuZipEncoder fed by submit_device, or stand-ins with the same interfaces)."""
+    zipfile_gpu.GpuZipEncoder fed by submit_device and, with check, deps.GpuElfParser and deps.GpuSymbolResolver, or
+    stand-ins with the same interfaces)."""
     srcs = [os.fspath(srcs)] if isinstance(srcs, (str, bytes, os.PathLike)) else [os.fspath(s) for s in srcs]
     dst = os.fspath(dst)
     check_prefix(prefix)
+    check = _check_engines(check, parser, resolver)
     if not srcs:
         raise ValueError("zip_tarballs: no source")
     for s in srcs:
@@ -293,6 +300,9 @@ def zip_with(srcs, dst, reader, indexer, stripper, encoder, prefix="", fallback_
         infos.append((None, zip_info(p, node, ref[1] if ref else 0, umask)))
         if ref is not None:
             items.append((i, ref))
+    report = None
+    if check is not None:
+        report = check_layer(check, [zi for _, zi in infos], dict(items), {}, None, parser, resolver)
 
     out_dir = os.path.dirname(dst) or "."
     os.makedirs(out_dir, exist_ok=True)
@@ -338,11 +348,49 @@ def zip_with(srcs, dst, reader, indexer, stripper, encoder, prefix="", fallback_
           "index": index, "inflate": reader.stats(), "strip": stripper.stats(), "deflate": encoder.stats()}
     st["kernel_ms"] = (st["inflate"].get("kernel_ms", 0.0) + index["kernel_ms"] + sum(st["strip"].values()) +
                        st["deflate"].get("kernel_ms", 0.0))
+    if report is not None:
+        st["check"] = report
     return st
 
 
+def _check_engines(check, parser, resolver):
+    """check validated before any source is read (deps.check_options), and the engines it needs present"""
+    if check is None:
+        return None
+    check = D.check_options(check)
+    if parser is None or (check.get("symbols") and resolver is None):
+        raise ValueError("check needs a parser, and a resolver with symbols=True")
+    return check
+
+
+def check_layer(check, infos, resident, wheel_members, decoder, parser, resolver):
+    """deps.check_entries(**check) over a zip before any of it is written: infos [ZipInfo] are its entries, resident
+    {entry index: (device address, size)} the entries whose bytes the writer holds on the device (the stripped
+    objects, the tar arena, the host upload) and wheel_members {entry index: (ZipInfo, (ZipFile, open file, size))}
+    the entries whose DEFLATE body is copied from a wheel, inflated by decoder when a closure reaches them.  Returns the
+    report check_zip gives for the zip, its stats with inflate_ms (those inflates only) and roots_reused (the roots
+    whose bytes were already on the device); raises deps.CheckFailed when it has problems."""
+    entries = [(i, zi.filename, None) for i, zi in enumerate(infos)]   # a symlink is written as a file entry
+    later = D.member_decoder(decoder, parser, wheel_members)
+    ms0 = decoder.stats().get("kernel_ms", 0.0) if decoder is not None else 0.0
+
+    def decode(keys, consume):
+        here = [k for k in keys if k in resident]
+        if here:
+            consume(here, [resident[k] for k in here])
+        rest = [k for k in keys if k not in resident]
+        return later(rest, consume) if rest else 0
+    report = D.check_entries(entries, decode, parser, resolver=resolver, **check)
+    st = report["stats"]
+    st["inflate_ms"] = decoder.stats().get("kernel_ms", 0.0) - ms0 if decoder is not None else 0.0
+    st["roots_reused"] = sum(1 for i, zi in enumerate(infos) if i in resident and Z.selected_for_strip(zi))
+    if report["problems"]:
+        raise D.CheckFailed(report)
+    return report
+
+
 def zip_tarballs(srcs, dst, prefix="", ctx=None, compresslevel=None, fallback_host_strip=True, tolerate_non_elf=False,
-                 piece_bytes=PIECE_BYTES, seek_table=False):
+                 piece_bytes=PIECE_BYTES, seek_table=False, check=None):
     """Write the Lambda zip `dst` of the package tarballs `srcs` (one .tar.gz path or a list), every shared object
     stripped, without unpacking them: entry for entry the zip that these passes give --
     `tarfile.open(src, "r:gz").extractall(tree / prefix, filter="fully_trusted")` for each source in order,
@@ -378,22 +426,39 @@ def zip_tarballs(srcs, dst, prefix="", ctx=None, compresslevel=None, fallback_ho
     Returns a stats dict: sources, members, entries, files, skipped_entries; selected, gpu, fallback, skipped; in_bytes
     / out_bytes (the stripped files before and after), file_bytes (every file entry's bytes), deflated_bytes (their
     bodies), tar_bytes_in, src_bytes, zip_bytes; uploaded_bytes / downloaded_bytes (everything that crossed the bus);
-    index, inflate, strip and deflate (the engines' stats) and kernel_ms, their kernel times summed.  There is no CPU
-    path: without a GPU this raises."""
+    index, inflate, strip and deflate (the engines' stats) and kernel_ms, their kernel times summed.
+
+    check (a dict of check_zip's keyword arguments: mount, arch, provided, max_versions, ld_library_path, symbols,
+    interpreter, runtime_libs) checks the zip before it is written, on the stripped objects where they lie on the
+    device (DESIGN.md section 9.10): stats["check"] is the report check_zip(dst, **check) would return, with stats
+    roots_reused added, and a report with problems raises deps.CheckFailed (its report attached) before dst is
+    created or replaced.  An unknown key or a refused value raises ValueError before any source is read.  There is
+    no CPU path: without a GPU this raises."""
     N.deflate_flags(compresslevel)
     check_prefix(prefix)
+    if check is not None:
+        D.check_options(check)
     own = False
     if ctx is None:
         ctx, own = T._default_context()
     try:
         with T.GpuTarReader(ctx) as reader, Z.GpuStripper(ctx) as stripper, \
                 Z.GpuZipEncoder(ctx, piece_bytes, compresslevel=compresslevel, host_buffers=False,
-                                seek_table=seek_table) as enc:
+                                seek_table=seek_table) as enc, _check_engine_set(ctx, check) as (parser, resolver):
             return zip_with(srcs, dst, reader, T.GpuTarIndex(ctx), stripper, enc, prefix, fallback_host_strip,
-                            tolerate_non_elf)
+                            tolerate_non_elf, check, parser, resolver)
     finally:
         if own:
             ctx.close()
+
+
+@contextlib.contextmanager
+def _check_engine_set(ctx, check):
+    """(GpuElfParser, GpuSymbolResolver) for check, each None where check does not need it"""
+    with contextlib.ExitStack() as stack:
+        parser = stack.enter_context(D.GpuElfParser(ctx)) if check is not None else None
+        resolver = stack.enter_context(D.GpuSymbolResolver(ctx)) if check is not None and check.get("symbols") else None
+        yield parser, resolver
 
 
 # ---- zip_build: prebuilt tarballs and wheels, pip's target install and the build script's clean-up ----------------
@@ -681,12 +746,15 @@ def _entry_info(path, node, size, umask):
 
 
 def build_with(dst, tarballs, wheels, reader, indexer, decoder, stripper, encoder, prefix="", keep_tests=(),
-               executable=sys.executable, fallback_host_strip=True, tolerate_non_elf=False):
+               executable=sys.executable, fallback_host_strip=True, tolerate_non_elf=False, check=None, parser=None,
+               resolver=None):
     """zip_build with the engines given (tarball.GpuTarReader, tarball.GpuTarIndex, zipfile_gpu.GpuUnzipDecoder,
-    zipfile_gpu.GpuStripper, zipfile_gpu.GpuZipEncoder fed by submit_device, or stand-ins with the same interfaces)."""
+    zipfile_gpu.GpuStripper, zipfile_gpu.GpuZipEncoder fed by submit_device and, with check, deps.GpuElfParser and
+    deps.GpuSymbolResolver, or stand-ins with the same interfaces)."""
     tarballs, wheels = [os.fspath(t) for t in tarballs], [os.fspath(w) for w in wheels]
     dst = os.fspath(dst)
     check_prefix(prefix)
+    check = _check_engines(check, parser, resolver)
     if not tarballs and not wheels:
         raise ValueError("zip_build: no tarball and no wheel")
     for s in tarballs + wheels:
@@ -716,6 +784,9 @@ def build_with(dst, tarballs, wheels, reader, indexer, decoder, stripper, encode
 
     c = {"gpu": 0, "fallback": 0, "skipped": skipped, "in_bytes": 0, "out_bytes": 0, "uploaded": 0}
     dev, host = {}, {}          # id(node) -> its bytes for the zip: a device ref / bytes to upload after the strip
+    # the decoder's output lives until its next run; the check's later rounds run it again, so with a check a member
+    # left unstripped in that output (a stored member, a non-ELF `*.so` under tolerate_non_elf) goes up with the host's
+    keep_decoded = check is None
 
     def host_fix(data, name):
         fixed = stripper.host_strip(data) if fallback_host_strip else None
@@ -744,7 +815,7 @@ def build_with(dst, tarballs, wheels, reader, indexer, decoder, stripper, encode
                     host[id(f)] = stripper.fetch(new)
             elif status == N.ST_NOT_ELF and tolerate_non_elf:
                 c["skipped"] += 1
-                if keep_on_device:
+                if keep_on_device and (keep_decoded or not isinstance(f, _WheelFile)):
                     dev[id(f)] = r
                 else:
                     host[id(f)] = stripper.fetch(r)
@@ -782,7 +853,7 @@ def build_with(dst, tarballs, wheels, reader, indexer, decoder, stripper, encode
                     host[key] = host_fix(data, zi.filename) if key in chosen_ids else data
                 elif key in chosen_ids:
                     pairs.append((f, got[key][1]))
-                elif whole:
+                elif whole and keep_decoded:
                     dev[key] = got[key][1]
                 else:
                     host[key] = stripper.fetch(got[key][1])
@@ -829,6 +900,11 @@ def build_with(dst, tarballs, wheels, reader, indexer, decoder, stripper, encode
                 infos.append((None, zi))
             else:
                 infos.append((None, _entry_info(p, node, 0, umask)))
+        report, unzip = None, decoder.stats()          # the build's decodes; the check's are in its report
+        if check is not None:
+            report = check_layer(check, [zi for _, zi in infos], dict(items),
+                                 {i: (node.member, sources[node.src - len(tarballs)]) for i, node in copied.items()},
+                                 decoder, parser, resolver)
 
         out_dir = os.path.dirname(dst) or "."
         os.makedirs(out_dir, exist_ok=True)
@@ -906,10 +982,12 @@ def build_with(dst, tarballs, wheels, reader, indexer, decoder, stripper, encode
           "uploaded_bytes": reader.uploaded + c["uploaded"] + stripper.uploaded,
           "downloaded_bytes": reader.downloaded + 16 * index["ranges"] + index["bytes"] + downloaded +
           stripper.downloaded,
-          "index": index, "inflate": reader.stats() if tarballs else {}, "unzip": decoder.stats(),
+          "index": index, "inflate": reader.stats() if tarballs else {}, "unzip": unzip,
           "strip": stripper.stats(), "deflate": encoder.stats()}
     st["kernel_ms"] = (st["inflate"].get("kernel_ms", 0.0) + index["kernel_ms"] + st["unzip"].get("kernel_ms", 0.0) +
                        sum(st["strip"].values()) + st["deflate"].get("kernel_ms", 0.0))
+    if report is not None:
+        st["check"] = report
     return st
 
 
@@ -925,7 +1003,7 @@ def _body_offset(f, zi):
 
 def zip_build(dst, tarballs=(), wheels=(), prefix="", keep_tests=(), executable=sys.executable, ctx=None,
               compresslevel=None, fallback_host_strip=True, tolerate_non_elf=False, piece_bytes=PIECE_BYTES,
-              seek_table=False):
+              seek_table=False, check=None):
     """Write the Lambda zip `dst` of a whole build -- prebuilt package tarballs and wheels -- as `lambdipy build`
     leaves it, without unpacking anything: entry for entry the zip these passes give, with T = tree / prefix:
     `tarfile.open(t, "r:gz").extractall(T, filter="fully_trusted")` for each tarball in order, `pip install --no-deps
@@ -963,18 +1041,26 @@ def zip_build(dst, tarballs=(), wheels=(), prefix="", keep_tests=(), executable=
 
     Returns zip_tarballs' stats dict with wheels, wheel_members, copied (members, bytes, file_bytes),
     generated_scripts, removed (the clean-up's matches per rule and the entries removed), skipped_items and unzip (the
-    decoder's stats) added.  There is no CPU path: without a GPU this raises."""
+    decoder's stats for the build) added.
+
+    check is zip_tarballs' (DESIGN.md section 9.10): the roots are checked where the strip left them, the tarballs'
+    files in the tar arena, and a wheel member that only a closure reaches (a `.libs/*.so.N`, whose body is otherwise
+    copied) is inflated by the same decoder for the check alone.  With a check, a wheel member left unstripped in the
+    decoder's output goes up with the files made on the host instead, since the check's inflates reuse that output.
+    There is no CPU path: without a GPU this raises."""
     N.deflate_flags(compresslevel)
     check_prefix(prefix)
+    if check is not None:
+        D.check_options(check)
     own = False
     if ctx is None:
         ctx, own = T._default_context()
     try:
         with T.GpuTarReader(ctx) as reader, Z.GpuUnzipDecoder(ctx) as dec, Z.GpuStripper(ctx) as stripper, \
                 Z.GpuZipEncoder(ctx, piece_bytes, compresslevel=compresslevel, host_buffers=False,
-                                seek_table=seek_table) as enc:
+                                seek_table=seek_table) as enc, _check_engine_set(ctx, check) as (parser, resolver):
             return build_with(dst, tarballs, wheels, reader, T.GpuTarIndex(ctx), dec, stripper, enc, prefix,
-                              keep_tests, executable, fallback_host_strip, tolerate_non_elf)
+                              keep_tests, executable, fallback_host_strip, tolerate_non_elf, check, parser, resolver)
     finally:
         if own:
             ctx.close()
@@ -982,7 +1068,9 @@ def zip_build(dst, tarballs=(), wheels=(), prefix="", keep_tests=(), executable=
 
 def main(argv=None):
     """python -m lambdipy_b200.layer DST [SRC ...] [--wheel WHL ...] [--keep-tests NAME ...] [--clean]
-    [--prefix python/] [--level 9] [--seek-table]"""
+    [--prefix python/] [--level 9] [--seek-table] [--check [the options of python -m lambdipy_b200.deps]]
+
+    With --check, exit status 1 when the check finds problems (no zip is written) and 2 on a refused input."""
     import argparse
     ap = argparse.ArgumentParser(prog="python -m lambdipy_b200.layer",
                                  description="write the Lambda zip of .tar.gz package assets, shared objects stripped, "
@@ -999,25 +1087,46 @@ def main(argv=None):
     ap.add_argument("--level", type=int, choices=[9], default=None, help="9: the optimal parse (smaller, slower)")
     ap.add_argument("--seek-table", action="store_true",
                     help="give multi-chunk members seek tables, with which the GPU reader decodes them without search")
+    ap.add_argument("--check", action="store_true",
+                    help="check that the shared objects will load on Lambda, as python -m lambdipy_b200.deps does, "
+                         "before the zip is written; on a problem no zip is written (the options below need it)")
+    check_dests = D.add_check_arguments(ap)
     args = ap.parse_args(argv)
     if not args.srcs and not args.wheel:
         ap.error("give at least one tarball or --wheel")
-    if args.wheel or args.clean:
-        st = zip_build(args.dst, args.srcs, args.wheel, prefix=args.prefix, keep_tests=args.keep_tests,
-                       compresslevel=args.level, **ST.seek_kw(args.seek_table))
-        print("Layer zip: %s, %.1f MB from %d tarballs and %d wheels (%.1f MB), %d entries; %d bodies copied, %d "
-              "entries cleaned up; %d shared objects stripped (%d via host strip), %.1f MB -> %.1f MB"
-              % (args.dst, st["zip_bytes"] / 1e6, len(args.srcs), len(args.wheel), st["src_bytes"] / 1e6,
-                 st["entries"], st["copied"]["members"], st["removed"]["entries"], st["gpu"] + st["fallback"],
-                 st["fallback"], st["in_bytes"] / 1e6, st["out_bytes"] / 1e6))
-        return 0
-    if args.keep_tests:
-        ap.error("--keep-tests needs --clean or --wheel")
-    st = zip_tarballs(args.srcs, args.dst, prefix=args.prefix, compresslevel=args.level, **ST.seek_kw(args.seek_table))
-    print("Layer zip: %s, %.1f MB from %d tarballs (%.1f MB), %d entries; %d shared objects stripped (%d via host "
-          "strip), %.1f MB -> %.1f MB"
-          % (args.dst, st["zip_bytes"] / 1e6, len(args.srcs), st["src_bytes"] / 1e6, st["entries"],
-             st["gpu"] + st["fallback"], st["fallback"], st["in_bytes"] / 1e6, st["out_bytes"] / 1e6))
+    if not args.check and any(getattr(args, k) != ap.get_default(k) for k in check_dests):
+        ap.error("--mount, --arch, --provided, --max-version, --ld-library-path, --symbols, --interpreter and "
+                 "--runtime-lib need --check")
+    try:
+        kw = {"check": D.check_kwargs(args)} if args.check else {}
+        if args.wheel or args.clean:
+            st = zip_build(args.dst, args.srcs, args.wheel, prefix=args.prefix, keep_tests=args.keep_tests,
+                           compresslevel=args.level, **ST.seek_kw(args.seek_table), **kw)
+            print("Layer zip: %s, %.1f MB from %d tarballs and %d wheels (%.1f MB), %d entries; %d bodies copied, %d "
+                  "entries cleaned up; %d shared objects stripped (%d via host strip), %.1f MB -> %.1f MB"
+                  % (args.dst, st["zip_bytes"] / 1e6, len(args.srcs), len(args.wheel), st["src_bytes"] / 1e6,
+                     st["entries"], st["copied"]["members"], st["removed"]["entries"], st["gpu"] + st["fallback"],
+                     st["fallback"], st["in_bytes"] / 1e6, st["out_bytes"] / 1e6))
+        else:
+            if args.keep_tests:
+                ap.error("--keep-tests needs --clean or --wheel")
+            st = zip_tarballs(args.srcs, args.dst, prefix=args.prefix, compresslevel=args.level,
+                              **ST.seek_kw(args.seek_table), **kw)
+            print("Layer zip: %s, %.1f MB from %d tarballs (%.1f MB), %d entries; %d shared objects stripped (%d via "
+                  "host strip), %.1f MB -> %.1f MB"
+                  % (args.dst, st["zip_bytes"] / 1e6, len(args.srcs), st["src_bytes"] / 1e6, st["entries"],
+                     st["gpu"] + st["fallback"], st["fallback"], st["in_bytes"] / 1e6, st["out_bytes"] / 1e6))
+    except D.CheckFailed as e:
+        print("Layer zip: %s not written" % args.dst)
+        print(D.summary(e.report))
+        return 1
+    except (OSError, ValueError, zipfile.BadZipFile) as e:
+        if not args.check:
+            raise
+        print("error: %s" % e, file=sys.stderr)
+        return 2
+    if args.check:
+        print(D.summary(st["check"]))
     return 0
 
 
