@@ -558,7 +558,17 @@ int lb2_elf_deps(lb2_ctx *ctx, const uint64_t *d_ptrs, const uint64_t *sizes, ui
  *
  * lb2_syms_names: the strings of misses[0 .. n): for miss i, h_pool[offsets[i] ..] holds its symbol name, the name of
  * the version it asks for and the file of that version need, each followed by a NUL (empty when not versioned).
- * LB2_E_CAPACITY when pool_cap is too small (*pool_bytes says what is needed). */
+ * LB2_E_CAPACITY when pool_cap is too small (*pool_bytes says what is needed).
+ *
+ * lb2_syms_find: what dlsym(handle, name) returns, for names the host gives (deps.check_zip(python=...) looks up each
+ * extension module's PyInit_* this way).  Query q looks the name h_names[name_off ..+ name_len) up in the scope
+ * scope[scope_off ..+ scope_len) (object ids: the handle's local scope, the object and its DT_NEEDED closure breadth
+ * first), one warp per query, with the rules of lb2_syms_resolve for an unversioned lookup under
+ * DL_LOOKUP_RETURN_NEWEST: a definition at versym index 0 or 1 is taken, one at index 2 or above only when it is not
+ * hidden and the object's single such candidate.  found[q] is the first object in scope order that defines it: its id,
+ * the symbol's index, st_info, st_other and versym (0 without DT_VERSYM); obj is LB2_SYM_NOT_FOUND when none does.
+ * Only the names go up and only found[] comes down; stats.resolve_ms times the kernel.  LB2_E_ARG for a query outside
+ * the name pool or the scope array, or a scope entry that is not an object id. */
 #define LB2_SYM_OK 0
 #define LB2_SYM_NOT_ELF 1
 #define LB2_SYM_UNSUPPORTED 2        /* ELF32, big-endian, or DT_REL relocations                                     */
@@ -583,6 +593,16 @@ typedef struct lb2_sym_job {
 typedef struct lb2_sym_miss {
   uint32_t job, ref;
 } lb2_sym_miss;
+#define LB2_SYM_NOT_FOUND 0xffffffffu
+typedef struct lb2_sym_query {
+  uint32_t scope_off, scope_len;     /* the scope: scope[scope_off ..+ scope_len)                                  */
+  uint32_t name_off, name_len;       /* the name: h_names[name_off ..+ name_len), no NUL needed                     */
+} lb2_sym_query;
+typedef struct lb2_sym_found {
+  uint32_t obj, sym;                 /* the defining object's id (LB2_SYM_NOT_FOUND: none) and the symbol's index   */
+  uint8_t info, other;               /* its st_info, st_other                                                       */
+  uint16_t versym;                   /* its .gnu.version entry, 0 without DT_VERSYM                                 */
+} lb2_sym_found;
 typedef struct lb2_syms_stats {
   uint64_t bytes_up, bytes_down;     /* host-device bytes of the call                                              */
   uint64_t references, lookups;      /* references indexed or resolved; scope entries probed                        */
@@ -599,6 +619,8 @@ int lb2_syms_resolve(lb2_syms *s, const lb2_sym_job *jobs, uint32_t n_jobs, cons
                      uint32_t *n_misses, lb2_syms_stats *stats);
 int lb2_syms_names(lb2_syms *s, const lb2_sym_job *jobs, uint32_t n_jobs, const lb2_sym_miss *misses, uint32_t n,
                    uint64_t *offsets, void *h_pool, uint64_t pool_cap, uint64_t *pool_bytes, lb2_syms_stats *stats);
+int lb2_syms_find(lb2_syms *s, const lb2_sym_query *queries, uint32_t n, const uint32_t *scope, uint32_t n_scope,
+                  const void *h_names, uint64_t names_bytes, lb2_sym_found *found, lb2_syms_stats *stats);
 
 #ifdef __cplusplus
 }

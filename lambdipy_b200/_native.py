@@ -32,7 +32,7 @@ EXPORTS = [
     "lb2_inflate_device_output", "lb2_memcpy_d2d", "lb2_gzip_submit_device", "lb2_tar_index",
     "lb2_gzip_chunk_sizes", "lb2_inflate_run_table", "lb2_zip_chunk_sizes", "lb2_unzip_run_table",
     "lb2_cleanup_tests_removed", "lb2_elf_deps",
-    "lb2_syms_create", "lb2_syms_destroy", "lb2_syms_index", "lb2_syms_resolve", "lb2_syms_names",
+    "lb2_syms_create", "lb2_syms_destroy", "lb2_syms_index", "lb2_syms_resolve", "lb2_syms_names", "lb2_syms_find",
 ]
 TAR_STOP_ZERO, TAR_STOP_BAD_HEADER, TAR_STOP_END, TAR_STOP_UNSUPPORTED = 1, 2, 3, 4
 ZIP_CONTINUES, ZIP_MORE = 1, 2
@@ -40,6 +40,7 @@ ELF_OK, ELF_NOT_ELF, ELF_UNSUPPORTED, ELF_STATIC, ELF_MALFORMED = 0, 1, 2, 3, 4 
 ELF_REC_SONAME, ELF_REC_NEEDED, ELF_REC_RPATH, ELF_REC_RUNPATH = 1, 2, 3, 4  # LB2_ELF_REC_*
 ELF_REC_VERNEED_FILE, ELF_REC_VERNEED_VERSION, ELF_REC_VERDEF = 5, 6, 7
 SYM_OK, SYM_UNSUPPORTED, SYM_MALFORMED = 0, 2, 4  # LB2_SYM_* (the LB2_ELF_* values)
+SYM_NOT_FOUND = 0xFFFFFFFF  # LB2_SYM_NOT_FOUND
 DEFLATE_BEST = 1  # LB2_DEFLATE_BEST
 
 
@@ -201,6 +202,15 @@ class SymMiss(C.Structure):
     _fields_ = [("job", C.c_uint32), ("ref", C.c_uint32)]
 
 
+class SymQuery(C.Structure):
+    _fields_ = [("scope_off", C.c_uint32), ("scope_len", C.c_uint32), ("name_off", C.c_uint32), ("name_len", C.c_uint32)]
+
+
+class SymFound(C.Structure):
+    _fields_ = [("obj", C.c_uint32), ("sym", C.c_uint32), ("info", C.c_uint8), ("other", C.c_uint8),
+                ("versym", C.c_uint16)]
+
+
 class SymsStats(C.Structure):
     _fields_ = [("bytes_up", C.c_uint64), ("bytes_down", C.c_uint64), ("references", C.c_uint64),
                 ("lookups", C.c_uint64), ("arena_bytes", C.c_uint64), ("index_ms", C.c_float),
@@ -358,6 +368,9 @@ def load():
     lib.lb2_syms_names.argtypes = [vp, C.POINTER(SymJob), C.c_uint32, C.POINTER(SymMiss), C.c_uint32, u64p, vp,
                                    C.c_uint64, u64p, C.POINTER(SymsStats)]
     lib.lb2_syms_names.restype = C.c_int
+    lib.lb2_syms_find.argtypes = [vp, C.POINTER(SymQuery), C.c_uint32, u32p, C.c_uint32, vp, C.c_uint64,
+                                  C.POINTER(SymFound), C.POINTER(SymsStats)]
+    lib.lb2_syms_find.restype = C.c_int
     _lib = lib
     return lib
 

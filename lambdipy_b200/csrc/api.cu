@@ -1741,6 +1741,8 @@ int lb2_elf_deps(lb2_ctx *ctx, const uint64_t *d_ptrs, const uint64_t *sizes, ui
 #include "elf_syms.cuh"
 static_assert(sizeof(lb2_sym_object) == sizeof(elfs::Object), "the index kernels write lb2_sym_object records");
 static_assert(sizeof(lb2_sym_job) == sizeof(elfs::Job) && sizeof(lb2_sym_miss) == sizeof(elfs::Miss), "resolve records");
+static_assert(sizeof(lb2_sym_query) == sizeof(elfs::Query) && sizeof(lb2_sym_found) == sizeof(elfs::Found) &&
+              LB2_SYM_NOT_FOUND == elfs::NOT_FOUND, "find records");
 
 struct lb2_syms {
   lb2_ctx *ctx = nullptr;
@@ -2028,6 +2030,56 @@ int lb2_syms_names(lb2_syms *s, const lb2_sym_job *jobs, uint32_t n_jobs, const 
   if (e != cudaSuccess) { ctx->err = std::string("lb2_syms_names: ") + cudaGetErrorString(e); return LB2_E_CUDA; }
   if (stats) *stats = st;
   if (!fits) { ctx->err = "lb2_syms_names: the strings exceed pool_cap (*pool_bytes needed)"; return LB2_E_CAPACITY; }
+  return LB2_OK;
+}
+
+int lb2_syms_find(lb2_syms *s, const lb2_sym_query *queries, uint32_t n, const uint32_t *scope, uint32_t n_scope,
+                  const void *h_names, uint64_t names_bytes, lb2_sym_found *found, lb2_syms_stats *stats) {
+  if (!s) return LB2_E_ARG;
+  lb2_ctx *ctx = s->ctx;
+  const uint64_t n_obj = s->objs.size();
+  if ((n && (!queries || !found)) || (n_scope && !scope) || (names_bytes && !h_names)) {
+    ctx->err = "NULL argument";
+    return LB2_E_ARG;
+  }
+  for (uint32_t i = 0; i < n_scope; i++)
+    if (scope[i] >= n_obj) { ctx->err = "lb2_syms_find: a scope entry is not an object id"; return LB2_E_ARG; }
+  for (uint32_t q = 0; q < n; q++)
+    if (queries[q].scope_off > n_scope || queries[q].scope_len > n_scope - queries[q].scope_off ||
+        queries[q].name_off > names_bytes || queries[q].name_len > names_bytes - queries[q].name_off) {
+      ctx->err = "lb2_syms_find: a query outside the scope array or the name pool";
+      return LB2_E_ARG;
+    }
+  lb2_syms_stats st{};
+  if (!n) { if (stats) *stats = st; return LB2_OK; }
+  CK(cudaSetDevice(ctx->device));
+  const uint64_t ob = sizeof(lb2_sym_object) * n_obj, qb = sizeof(lb2_sym_query) * (uint64_t)n, sb = 4ull * n_scope,
+                 fb = sizeof(lb2_sym_found) * (uint64_t)n;
+  uint64_t o[6] = {0};  // offsets: objects, queries, scope, names, found, end
+  const uint64_t sz[5] = {ob, qb, sb, names_bytes, fb};
+  for (int k = 0; k < 5; k++) o[k + 1] = (o[k] + sz[k] + 15) & ~15ull;
+  SymScratch w(o[5]);
+  cudaError_t &e = w.e;
+  cudaStream_t q = ctx->stream;
+  const void *src[4] = {s->objs.data(), queries, scope, h_names};
+  for (int k = 0; k < 4; k++)
+    if (e == cudaSuccess && sz[k]) e = cudaMemcpyAsync(w.d + o[k], src[k], sz[k], cudaMemcpyHostToDevice, q);
+  st.bytes_up = ob + qb + sb + names_bytes;
+  if (e == cudaSuccess) e = cudaEventRecord(w.ev[0], q);
+  if (e == cudaSuccess) {
+    launch_syms_find(w.d + o[0], reinterpret_cast<const elfs::Query *>(w.d + o[1]), n,
+                     reinterpret_cast<const uint32_t *>(w.d + o[2]), w.d + o[3], reinterpret_cast<elfs::Found *>(w.d + o[4]), q);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaEventRecord(w.ev[1], q);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(found, w.d + o[4], fb, cudaMemcpyDeviceToHost, q);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(q);
+  st.bytes_down = fb;
+  st.resolve_ms = w.ms(0, 1);
+  if (e != cudaSuccess) { ctx->err = std::string("lb2_syms_find: ") + cudaGetErrorString(e); return LB2_E_CUDA; }
+  st.references = n;
+  st.arena_bytes = s->total;
+  if (stats) *stats = st;
   return LB2_OK;
 }
 

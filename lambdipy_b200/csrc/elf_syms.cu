@@ -6,13 +6,15 @@
 // entries marks the referenced undefined symbols in each object's bitmap; a count pass (one warp per object) counts
 // and checks them, the host places the Ref arrays, and a write pass compacts the bitmap into them.  Resolve: one warp
 // per (reference, scope); the lanes look the symbol up in 32 objects of the scope at a time and a ballot keeps the
-// first that defines it.
+// first that defines it.  Find: one warp per query, the same 32-at-a-time probe of a name the host uploaded.
 #include "lb2_common.cuh"
 #include "elf_syms.cuh"
 
 namespace lb2 {
 using SymJob = elfs::Job;
 using SymMiss = elfs::Miss;
+using SymQuery = elfs::Query;
+using SymFound = elfs::Found;
 namespace {
 using elfs::Object;
 using elfs::Ref;
@@ -213,6 +215,44 @@ __global__ void __launch_bounds__(32 * WARPS) lb2_syms_resolve_kernel(const Obje
   if (lane == 0 && probed) atomicAdd(lookups, probed);
 }
 
+// One warp per query: the name pool[name_off ..+ name_len) looked up as dlsym looks it up (newest) in scope[scope_off
+// ..+ scope_len); every lane hashes the name, then probes one scope entry of each 32.  The host has checked that
+// every query lies inside the pool and the scope array and that every scope entry is an object id.
+__global__ void __launch_bounds__(32 * WARPS) lb2_syms_find_kernel(const Object *objs, const SymQuery *queries, uint32_t n,
+                                                                   const uint32_t *scope, const uint8_t *pool,
+                                                                   SymFound *found) {
+  const uint32_t q = blockIdx.x * WARPS + threadIdx.x / 32, lane = threadIdx.x & 31;
+  if (q >= n) return;
+  const SymQuery qy = queries[q];
+  const uint8_t *name = pool + qy.name_off;
+  const uint32_t gnu = elfs::gnu_hash(name, qy.name_len), sysv = elfs::sysv_hash(name, qy.name_len);
+  int64_t sym = -1;
+  uint32_t at = 0;
+  for (uint32_t b = 0; b < qy.scope_len; b += 32) {
+    int64_t s = -1;
+    if (b + lane < qy.scope_len) {
+      const Object &d = objs[scope[qy.scope_off + b + lane]];
+      s = elfs::lookup_name(d, reinterpret_cast<const uint8_t *>(d.arena), name, qy.name_len, gnu, sysv, nullptr,
+                            nullptr, true);
+    }
+    const uint32_t m = __ballot_sync(0xFFFFFFFFu, s >= 0);
+    if (m) {
+      const int first = __ffs(m) - 1;
+      at = b + first;
+      sym = __shfl_sync(0xFFFFFFFFu, s, first);
+      break;
+    }
+  }
+  if (lane == 0) {
+    if (sym < 0) {
+      found[q] = SymFound{elfs::NOT_FOUND, 0, 0, 0, 0};
+    } else {
+      const uint32_t id = scope[qy.scope_off + at];
+      found[q] = elfs::found_at(id, objs[id], reinterpret_cast<const uint8_t *>(objs[id].arena), (uint32_t)sym);
+    }
+  }
+}
+
 // the strings of a missed reference: name, version name, version file, each followed by a NUL
 __device__ void miss_strings(const Object *objs, const SymJob *jobs, const SymMiss &m, const uint8_t *s[3], uint32_t len[3]) {
   const Object &o = objs[jobs[m.job].obj];
@@ -288,6 +328,12 @@ void launch_syms_names(const void *objs, const SymJob *jobs, const SymMiss *miss
     lb2_syms_names_count_kernel<<<(n + 127) / 128, 128, 0, s>>>(static_cast<const Object *>(objs), jobs, miss, n, len_or_off);
   else
     lb2_syms_names_write_kernel<<<(n + 127) / 128, 128, 0, s>>>(static_cast<const Object *>(objs), jobs, miss, n, len_or_off, pool);
+}
+
+void launch_syms_find(const void *objs, const SymQuery *queries, uint32_t n, const uint32_t *scope, const uint8_t *pool,
+                      SymFound *found, cudaStream_t s) {
+  if (n) lb2_syms_find_kernel<<<(n + WARPS - 1) / WARPS, 32 * WARPS, 0, s>>>(static_cast<const Object *>(objs), queries, n,
+                                                                             scope, pool, found);
 }
 
 }  // namespace lb2

@@ -15,6 +15,8 @@
 //    object's references, each with its GNU and SysV hash and its versym index.
 //  * lookup: one reference in one object: bloom filter, bucket, chain, name compare and check_match.  A warp takes
 //    32 objects of a scope at a time and a ballot keeps the first one in scope order that defines the symbol.
+//  * find: the same lookup of a name given by the host, as dlsym(handle, name) does it (elf/dl-sym.c: the handle's
+//    local scope, DL_LOOKUP_RETURN_NEWEST), for the PyInit_* export of a Python extension module.
 //
 // Bounds are elf_deps.cuh's: no byte outside [0, n) of an object is read; every table must map into a PT_LOAD's file
 // image and fit there; strings must end before DT_STRSZ; version chains are walked at most their count and n / 8 + 2
@@ -368,14 +370,18 @@ ED_HD bool same(const uint8_t *x, const uint8_t *y, uint64_t len) {
   return true;
 }
 
-// do_lookup_x for one object: the index of the symbol of d (arena block da) that the reference r of o (arena block
-// oa) binds to, or -1.  rv: ref_version(o, oa, r).
-ED_HD int64_t lookup(const Object &d, const uint8_t *da, const Object &o, const uint8_t *oa, const Ref &r, const Ver *rv) {
+// do_lookup_x for one object: the index of the symbol of d (arena block da) named name[0, len) (gnu / sysv: its
+// hashes) that check_match accepts, or -1.  rv: the version asked for, its name at rv_name, or null for an unversioned
+// lookup.  newest: DL_LOOKUP_RETURN_NEWEST (dlsym): an unversioned lookup counts a definition at versym index 2 or
+// above as a versioned candidate, where a relocation counts index 3 or above.  name is read only in [0, len).
+ED_HD int64_t lookup_name(const Object &d, const uint8_t *da, const uint8_t *name, uint32_t len, uint32_t gnu,
+                          uint32_t sysv, const Ver *rv, const uint8_t *rv_name, bool newest) {
   if (d.status != ST_OK || !d.nbucket || !d.nhash) return -1;
   const Tables t = tables(d);
-  const uint8_t *syms = da + t.sym, *dstr = da + t.str, *name = oa + tables(o).str + r.name;
+  const uint8_t *syms = da + t.sym, *dstr = da + t.str;
   const Ver *dver = reinterpret_cast<const Ver *>(da + t.ver);
   const bool versym = d.flags & F_VERSYM;
+  const uint32_t multi = newest ? 2 : 3;
   int64_t versioned = -1;
   uint32_t num_versions = 0;
   // check_match without the binding test (do_lookup_x applies that to what check_match returns)
@@ -385,17 +391,17 @@ ED_HD int64_t lookup(const Object &d, const uint8_t *da, const Object &o, const 
     if ((rd(syms, s + 8, 8) == 0 && shndx != SHN_ABS && type != STT_TLS) || shndx == SHN_UNDEF) return false;
     if (!((1u << type) & ALLOWED_STT)) return false;
     const uint64_t nm = rd(syms, s, 4);
-    if (nm >= d.str_len || r.name_len > d.str_len - nm || !same(dstr + nm, name, r.name_len + 1ull)) return false;
+    // .dynstr's copy ends in a NUL one past str_len: the definition's name must end right after len bytes
+    if (nm >= d.str_len || len > d.str_len - nm || !same(dstr + nm, name, len) || dstr[nm + len]) return false;
     if (!versym) return true;
     const uint32_t vs = (uint32_t)rd(da + t.versym, 2 * i, 2), ndx = vs & 0x7fff;
     if (rv) {
       const Ver *dv = ndx < d.nver && (dver[ndx].flags & 1) ? dver + ndx : nullptr;
       const uint32_t dh = dv ? dv->hash : 0;
-      const bool name_eq = dv && dv->name_len == rv->name_len &&
-                           same(dstr + dv->name, oa + tables(o).str + rv->name, rv->name_len);
+      const bool name_eq = dv && dv->name_len == rv->name_len && same(dstr + dv->name, rv_name, rv->name_len);
       return !((dh != rv->hash || !name_eq) && ((rv->flags & 2) || dh || (vs & 0x8000)));
     }
-    if (ndx >= 3) {  // an unversioned reference: a non-default version counts only as the object's single one
+    if (ndx >= multi) {  // an unversioned lookup: a non-default version counts only as the object's single one
       if (!(vs & 0x8000) && num_versions++ == 0) versioned = (int64_t)i;
       return false;
     }
@@ -404,12 +410,12 @@ ED_HD int64_t lookup(const Object &d, const uint8_t *da, const Object &o, const 
   int64_t hit = -1;
   if (d.flags & F_GNU) {
     const uint8_t *h = da + t.hash;
-    const uint64_t word = rd(h, 16 + 8ull * ((r.gnu / 64) & (d.bloom_words - 1)), 8);
-    if (!((word >> (r.gnu % 64)) & (word >> ((r.gnu >> d.bloom_shift) % 64)) & 1)) return -1;
+    const uint64_t word = rd(h, 16 + 8ull * ((gnu / 64) & (d.bloom_words - 1)), 8);
+    if (!((word >> (gnu % 64)) & (word >> ((gnu >> d.bloom_shift) % 64)) & 1)) return -1;
     const uint8_t *bucket = h + 16 + 8ull * d.bloom_words, *chain = bucket + 4ull * d.nbucket;
-    for (uint64_t i = rd(bucket, 4ull * (r.gnu % d.nbucket), 4); i && i < d.nhash; i++) {
+    for (uint64_t i = rd(bucket, 4ull * (gnu % d.nbucket), 4); i && i < d.nhash; i++) {
       const uint32_t c = (uint32_t)rd(chain, 4 * (i - d.symoffset), 4);
-      if (((c ^ r.gnu) >> 1) == 0 && check(i)) {
+      if (((c ^ gnu) >> 1) == 0 && check(i)) {
         hit = (int64_t)i;
         break;
       }
@@ -418,7 +424,7 @@ ED_HD int64_t lookup(const Object &d, const uint8_t *da, const Object &o, const 
   } else {
     const uint8_t *h = da + t.hash, *bucket = h + 8, *chain = bucket + 4ull * d.nbucket;
     uint64_t steps = 0;
-    for (uint64_t i = rd(bucket, 4ull * (r.sysv % d.nbucket), 4); i && i < d.nhash && steps < d.nhash;
+    for (uint64_t i = rd(bucket, 4ull * (sysv % d.nbucket), 4); i && i < d.nhash && steps < d.nhash;
          i = rd(chain, 4 * i, 4), steps++)
       if (check(i)) {
         hit = (int64_t)i;
@@ -431,6 +437,30 @@ ED_HD int64_t lookup(const Object &d, const uint8_t *da, const Object &o, const 
   if (!(bind == STB_GLOBAL || bind == STB_WEAK || bind == STB_GNU_UNIQUE)) return -1;
   if (vis == 1 || vis == 2) return -1;  // STV_INTERNAL, STV_HIDDEN
   return hit;
+}
+
+// lookup_name for the reference r of o (arena block oa), as a relocation looks it up.  rv: ref_version(o, oa, r).
+ED_HD int64_t lookup(const Object &d, const uint8_t *da, const Object &o, const uint8_t *oa, const Ref &r, const Ver *rv) {
+  const uint8_t *ostr = oa + tables(o).str;
+  return lookup_name(d, da, ostr + r.name, r.name_len, r.gnu, r.sysv, rv, rv ? ostr + rv->name : nullptr, false);
+}
+
+// find: the first object of scope[scope_off ..+ scope_len) (lb2_sym_query) that defines the name pool[name_off ..+
+// name_len) for dlsym; Found {obj, sym, st_info, st_other, versym} of it, obj NOT_FOUND when none does
+constexpr uint32_t NOT_FOUND = 0xffffffffu;
+struct Query {
+  uint32_t scope_off, scope_len, name_off, name_len;
+};
+struct Found {
+  uint32_t obj, sym;
+  uint8_t info, other;
+  uint16_t versym;
+};
+// Found of the symbol sym of d (arena block da)
+ED_HD Found found_at(uint32_t id, const Object &d, const uint8_t *da, uint32_t sym) {
+  const Tables t = tables(d);
+  const uint8_t *e = da + t.sym + (uint64_t)sym * SYM;
+  return Found{id, sym, e[4], e[5], d.flags & F_VERSYM ? (uint16_t)rd(da + t.versym, 2ull * sym, 2) : (uint16_t)0};
 }
 
 }  // namespace elfs

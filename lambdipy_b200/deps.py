@@ -4,7 +4,7 @@ shared object the zip's `import`s would load, on the GPU where the zip reader le
 
     python -m lambdipy_b200.deps ZIP [--mount DIR] [--arch x86_64|arm64] [--provided NAME]...
                                      [--max-version GLIBC_2.26]... [--ld-library-path P] [--json]
-                                     [--symbols [--interpreter FILE]... [--runtime-lib DIR]...]
+                                     [--symbols [--interpreter FILE]... [--runtime-lib DIR]...] [--python 3.N]
 
 A layer fails at the first `import` when a shared object cannot load: a DT_NEEDED library that neither the zip nor
 the runtime has, a symbol version newer than the runtime's, an object for the other architecture.  The check finds
@@ -39,6 +39,13 @@ objects followed by the root's closure (lb2_syms_*; DESIGN.md section 9.9).  Thi
 extension module built against another version of a library the zip carries.  Only counts and the failed lookups come
 back from the device.
 
+With python="3.N" (--python) the check also restates CPython's import finder (importlib's PathFinder and FileFinder)
+over the zip's tree on Lambda's sys.path and classes every `*.so` under it: an extension module the finder loads, a
+file it shadows, a build for another Python (a `cpython-3M` / `pypy` tag the target does not load) or a library.
+Each module's `PyInit_<name>` is looked up on the GPU as dlsym looks it up in the module's own load scope
+(lb2_syms_find; DESIGN.md section 9.11).  This finds `No module named ...` of a wheel built for another Python and
+`dynamic module does not define module export function` of a renamed extension before the upload.
+
 The check runs over entries (check_entries): check_with builds them from a zip's central directory, and the layer
 writers (layer.zip_build / zip_tarballs with check=...) from the entries of the zip they are about to write, with the
 bytes they already hold on the device (DESIGN.md section 9.10)."""
@@ -70,6 +77,13 @@ BATCH_BYTES = Z.BATCH_BYTES
 _VERSION = re.compile(r"^([A-Za-z][A-Za-z0-9]*)_(\d+(?:\.\d+)*)$")
 VER_FLG_WEAK = 2
 CLASS_IN_ZIP, CLASS_RUNTIME, CLASS_INTERPRETER = 0, 1, 2  # where a reference's definition was found
+PYTHON_VERSIONS = tuple("3.%d" % m for m in range(8, 15))
+# Lambda's sys.path entries a zip can fill, in order, from AWS's runtime documentation (/var/task, then a layer's
+# python/lib/python3.N/site-packages and python/); nobody has checked it against a runtime image here, so the report
+# echoes it.  The runtime's own entries come after these and are not modelled.
+LAMBDA_PYTHON_PATH = ("/var/task", "/opt/python/lib/python{version}/site-packages", "/opt/python")
+TRIPLETS = {"x86_64": "x86_64-linux-gnu", "arm64": "aarch64-linux-gnu"}
+_PY_TAG = re.compile(r"^([^.]+)\.((?:cpython-|pypy)[^.]*)\.so$")  # stem.TAG.so: an extension built for some Python
 
 
 class GpuElfParser:
@@ -141,7 +155,8 @@ class GpuSymbolResolver:
     into the resolver's device arena while the object is still there and returns [(id, status, references)];
     resolve(jobs, scope, classes) looks every reference of jobs' objects up in their scopes and returns ([(in_zip,
     runtime, interpreter) per job], [(job, reference) found nowhere, sorted]); names(jobs, misses) gives [(name, version,
-    version file)] of misses.  uploaded / downloaded count the bytes that crossed the bus."""
+    version file)] of misses; find(queries, scope) looks names up as dlsym does.  uploaded / downloaded count the
+    bytes that crossed the bus."""
 
     def __init__(self, ctx):
         self._ctx, h = ctx, C.c_void_p()
@@ -149,7 +164,8 @@ class GpuSymbolResolver:
         self._h = h
         self.uploaded = self.downloaded = 0
         self._miss_cap = 1 << 12
-        self._stats = {"index_ms": 0.0, "refs_ms": 0.0, "resolve_ms": 0.0, "references": 0, "lookups": 0}
+        self._stats = {"index_ms": 0.0, "refs_ms": 0.0, "resolve_ms": 0.0, "references": 0, "lookups": 0,
+                       "find_ms": 0.0, "find_queries": 0}
 
     def _account(self, st):
         self.uploaded += st.bytes_up
@@ -213,6 +229,22 @@ class GpuSymbolResolver:
         raw = pool.raw
         return [tuple(x.decode("utf-8", "surrogateescape") for x in raw[offs[i]:].split(b"\0", 3)[:3]) for i in range(n)]
 
+    def find(self, queries, scope):
+        """dlsym of names in scopes: queries [(scope_off, scope_len, name bytes)] over scope (resolver ids) ->
+        [(id of the first object defining it or None, symbol index, st_info, st_other, versym)]"""
+        n = len(queries)
+        if not n:
+            return []
+        cq, pool, found = find_arrays(queries)
+        cs, st = (C.c_uint32 * max(len(scope), 1))(*scope), N.SymsStats()
+        rc = self._ctx.lib.lb2_syms_find(self._h, cq, n, cs, len(scope), pool, len(pool), found, C.byref(st))
+        self._ctx.check(rc)
+        self.uploaded += st.bytes_up
+        self.downloaded += st.bytes_down
+        self._stats["find_ms"] += st.resolve_ms
+        self._stats["find_queries"] += n
+        return found_records(found, n)
+
     def stats(self):
         return dict(self._stats)
 
@@ -226,6 +258,20 @@ class GpuSymbolResolver:
 
     def __exit__(self, *exc):
         self.close()
+
+
+def find_arrays(queries):
+    """(lb2_sym_query array, name pool bytes, lb2_sym_found array) of find's queries [(scope_off, scope_len, name)]"""
+    cq, at = (N.SymQuery * max(len(queries), 1))(), 0
+    for i, (off, ln, name) in enumerate(queries):
+        cq[i] = N.SymQuery(off, ln, at, len(name))
+        at += len(name)
+    return cq, b"".join(name for _, _, name in queries), (N.SymFound * max(len(queries), 1))()
+
+
+def found_records(found, n):
+    """find's result of an lb2_sym_found array"""
+    return [(None if f.obj == N.SYM_NOT_FOUND else f.obj, f.sym, f.info, f.other, f.versym) for f in found[:n]]
 
 
 def decode(objs, recs, pool):
@@ -274,6 +320,7 @@ class _Tree:
     def __init__(self, entries, mount):
         self.mount = posixpath.normpath("/" + mount.strip("/")) if mount.strip("/") else "/"
         self.files, self.links, self.dirs, self.names = {}, {}, {self.mount}, {}
+        self._children = None
         d = self.mount
         while d != "/":
             d = posixpath.dirname(d)
@@ -299,6 +346,25 @@ class _Tree:
 
     def lookup(self, path):
         """the key of the regular file `path` ends at, symlinks followed, or None"""
+        got = self._walk(path)
+        return got[1] if got and got[0] == "file" else None
+
+    def directory(self, path):
+        """the directory `path` ends at, symlinks followed, or None"""
+        got = self._walk(path)
+        return got[1] if got and got[0] == "dir" else None
+
+    def children(self, d):
+        """the names in the directory d (a path directory() returned): files, links and directories"""
+        if self._children is None:
+            self._children = {}
+            for p in list(self.files) + list(self.links) + list(self.dirs):
+                if p != "/":
+                    self._children.setdefault(posixpath.dirname(p), set()).add(posixpath.basename(p))
+        return self._children.get(d, set())
+
+    def _walk(self, path):
+        """("file", key) or ("dir", its path) where `path` ends, symlinks followed, or None"""
         parts, i, cur, hops = [x for x in path.split("/") if x], 0, [], SYMLINK_HOPS
         while i < len(parts):
             comp = parts[i]
@@ -320,12 +386,12 @@ class _Tree:
                 continue
             last = i + 1 == len(parts) or all(x in ("", ".") for x in parts[i + 1:])
             if p in self.files:
-                return self.files[p] if last else None
+                return ("file", self.files[p]) if last else None
             if p not in self.dirs:
                 return None
             cur.append(comp)
             i += 1
-        return None
+        return "dir", "/" + "/".join(cur)
 
 
 def _version_key(v):
@@ -423,7 +489,8 @@ class _Model:
         return loaded, resolutions, pending
 
 
-CHECK_KEYS = ("mount", "arch", "provided", "max_versions", "ld_library_path", "symbols", "interpreter", "runtime_libs")
+CHECK_KEYS = ("mount", "arch", "provided", "max_versions", "ld_library_path", "symbols", "interpreter", "runtime_libs",
+              "python")
 
 
 class CheckFailed(Exception):
@@ -450,7 +517,8 @@ def _ceilings(arch, max_versions):
 
 def check_options(check):
     """check_zip's keyword arguments in the dict `check`, refused as check_with refuses them: ValueError for a key that
-    is not one of CHECK_KEYS, an unknown arch or a max_versions value that is not a dotted version"""
+    is not one of CHECK_KEYS, an unknown arch, a max_versions value that is not a dotted version or a python version
+    that is not one of PYTHON_VERSIONS"""
     if not isinstance(check, dict):
         raise ValueError("check=%r: expected a dict of check_zip's keyword arguments" % (check,))
     unknown = sorted(set(check) - set(CHECK_KEYS))
@@ -458,6 +526,7 @@ def check_options(check):
         raise ValueError("check: unknown key(s) %s; expected some of %s" % (", ".join(map(repr, unknown)),
                                                                          ", ".join(CHECK_KEYS)))
     _ceilings(check.get("arch", "x86_64"), check.get("max_versions"))
+    python_version(check.get("python"))
     return dict(check)
 
 
@@ -493,15 +562,16 @@ def member_decoder(decoder, parser, members, batch_bytes=BATCH_BYTES):
 
 def check_entries(entries, decode, parser, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVIDED,
                   max_versions=None, ld_library_path=LAMBDA_LD_LIBRARY_PATH, *, symbols=False, interpreter=(),
-                  runtime_libs=(), resolver=None, python_names=True):
+                  runtime_libs=(), resolver=None, python_names=True, python=None):
     """The check over the entries of a zip: entries [(key, name, link)] (an opaque hashable key, the entry's name, a
     symlink's target or None), in the zip's order.  decode(keys, consume) puts the regular files of a round on the
     device: it calls consume(part, refs) once or more, part a list of the keys and refs their (device address, size),
     valid until consume returns, and returns the bytes it uploaded.  The report has no inflate_ms: the caller knows
     what its decode step cost."""
-    if symbols and resolver is None:
-        raise ValueError("symbols=True needs a resolver")
+    if (symbols or python) and resolver is None:
+        raise ValueError("symbols=True and python need a resolver")
     ceilings = _ceilings(arch, max_versions)
+    python_version(python)
     sym_ids = {}
     tree = _Tree(entries, mount)
     path_of = {}
@@ -513,7 +583,7 @@ def check_entries(entries, decode, parser, mount="/var/task", arch="x86_64", pro
     model = _Model(tree, objs, arch, provided, ld_library_path)
 
     def consume(keys, refs):
-        if symbols:  # before parse(), which frees the uploads
+        if symbols or python:  # before parse(), which frees the uploads
             for key, got in zip(keys, resolver.index(refs)):
                 sym_ids[key] = got
         for key, (status, machine, records) in zip(keys, parser.parse(refs)):
@@ -533,21 +603,26 @@ def check_entries(entries, decode, parser, mount="/var/task", arch="x86_64", pro
     report["stats"] = {"members": len(entries), "roots": len(roots), "objects": len(objs), "rounds": rounds,
                        "bytes_up": uploaded + parser.uploaded, "bytes_down": parser.downloaded,
                        "parse_ms": parser.stats().get("kernel_ms", 0.0)}
+    counted = (0, 0)
     if symbols:
         _Symbols(tree, roots, objs, model, path_of, sym_ids, parser, resolver, provided, interpreter, runtime_libs,
                  python_names).check(report)
+        counted = (resolver.uploaded, resolver.downloaded)
+    if python:
+        _imports(report, tree, roots, objs, model, path_of, sym_ids, resolver, python, arch, counted)
     return report
 
 
 def check_with(zip_path, decoder, parser, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVIDED,
                max_versions=None, ld_library_path=LAMBDA_LD_LIBRARY_PATH, batch_bytes=BATCH_BYTES, *, symbols=False,
-               interpreter=(), runtime_libs=(), resolver=None, python_names=True):
-    """check_zip with the engines given (GpuUnzipDecoder, GpuElfParser and, with symbols=True, GpuSymbolResolver, or
-    stand-ins with the same interfaces).  python_names=False turns off the rule that counts an unresolved Py* / _Py*
-    name as the interpreter's when no interpreter is given."""
-    if symbols and resolver is None:
-        raise ValueError("symbols=True needs a resolver")
+               interpreter=(), runtime_libs=(), resolver=None, python_names=True, python=None):
+    """check_zip with the engines given (GpuUnzipDecoder, GpuElfParser and, with symbols=True or python,
+    GpuSymbolResolver, or stand-ins with the same interfaces).  python_names=False turns off the rule that counts an
+    unresolved Py* / _Py* name as the interpreter's when no interpreter is given."""
+    if (symbols or python) and resolver is None:
+        raise ValueError("symbols=True and python need a resolver")
     _ceilings(arch, max_versions)
+    python_version(python)
     with zipfile.ZipFile(zip_path) as zf, open(zip_path, "rb") as src:
         src.seek(0, os.SEEK_END)
         source = (zf, src, src.tell())
@@ -558,7 +633,7 @@ def check_with(zip_path, decoder, parser, mount="/var/task", arch="x86_64", prov
         decode = member_decoder(decoder, parser, {i: (zi, source) for i, zi in enumerate(infos)}, batch_bytes)
         report = check_entries(entries, decode, parser, mount, arch, provided, max_versions, ld_library_path,
                                symbols=symbols, interpreter=interpreter, runtime_libs=runtime_libs, resolver=resolver,
-                               python_names=python_names)
+                               python_names=python_names, python=python)
     report["stats"]["inflate_ms"] = decoder.stats().get("kernel_ms", 0.0)
     return report
 
@@ -804,9 +879,174 @@ class _Symbols:
                    "symbols_skipped": skipped})
 
 
+def python_version(python):
+    """python, refused unless None or one of PYTHON_VERSIONS ("3.8" .. "3.14"; free-threaded builds are not)"""
+    if python is not None and python not in PYTHON_VERSIONS:
+        raise ValueError("python=%r: expected one of %s" % (python, ", ".join(PYTHON_VERSIONS)))
+    return python
+
+
+def export_name(module):
+    """the PyInit_* name CPython looks up for the extension module `module` (importdl.c get_encoded_name and
+    dynload_shlib.c: the last dotted component, punycode with '-' as '_' and the PyInitU prefix when it is not ASCII,
+    cut to 200 bytes)"""
+    short = module.rsplit(".", 1)[-1]
+    try:
+        prefix, enc = b"PyInit", short.encode("ascii")
+    except UnicodeEncodeError:
+        prefix, enc = b"PyInitU", short.encode("punycode")
+    return prefix + b"_" + enc.replace(b"-", b"_")[:200]
+
+
+class _Finder:
+    """CPython's PathFinder with FileFinders of the target's loaders (importlib._bootstrap_external,
+    _get_supported_file_loaders) over the tree: the extension suffixes, then .py, then .pyc"""
+
+    def __init__(self, tree, version, arch):
+        self.tree = tree
+        self.ext = [".cpython-3%s-%s.so" % (version.split(".")[1], TRIPLETS[arch]), ".abi3.so", ".so"]
+        self.suffixes = self.ext + [".py", ".pyc"]
+        self.path = [p.format(version=version) for p in LAMBDA_PYTHON_PATH]
+        m = tree.mount
+        self.entries = [p for p in self.path if m == "/" or p == m or p.startswith(m + "/")]
+        self._specs = {}
+
+    def _in_dir(self, d, tail):
+        """FileFinder(d).find_spec(tail): (origin, None) for a module, (origin, [dir]) for a regular package,
+        (None, [dir]) for a namespace portion, or None"""
+        cd = self.tree.directory(d)
+        if cd is None:
+            return None
+        names, base, namespace = self.tree.children(cd), d + "/" + tail, False
+        if tail in names:
+            for suffix in self.suffixes:
+                if self.tree.lookup(base + "/__init__" + suffix) is not None:
+                    return base + "/__init__" + suffix, [base]
+            namespace = self.tree.directory(base) is not None
+        for suffix in self.suffixes:
+            if tail + suffix in names and self.tree.lookup(d + "/" + tail + suffix) is not None:
+                return d + "/" + tail + suffix, None
+        return (None, [base]) if namespace else None
+
+    def find(self, module):
+        """(origin or None, __path__ or None) of the dotted name `module` as `import` finds it, or None"""
+        if module not in self._specs:
+            parent, _, tail = module.rpartition(".")
+            search = self.entries
+            if parent:
+                spec = self.find(parent)
+                search = spec[1] if spec else None
+            found, portions = None, []
+            for d in search or ():
+                got = self._in_dir(d, tail)
+                if got and got[0] is not None:
+                    found = got
+                    break
+                portions += got[1] if got else []
+            self._specs[module] = found or ((None, portions) if portions else None)
+        return self._specs[module]
+
+    def name(self, path):
+        """(dotted module name, suffix, tag) of the file `path` under a path entry: tag None when its suffix is one of
+        the target's, else the other Python's tag; None when no importable name fits it"""
+        for e in self.entries:
+            if not path.startswith(e + "/"):
+                continue
+            parts = path[len(e) + 1:].split("/")
+            base, tag = parts.pop(), None
+            suffix = next((x for x in self.ext if base.endswith(x) and base[:-len(x)].isidentifier()), None)
+            if suffix is not None:
+                stem = base[:-len(suffix)]
+            else:
+                m = _PY_TAG.match(base)
+                if not m:
+                    return None
+                stem, tag, suffix = m.group(1), m.group(2), "." + m.group(2) + ".so"
+            parts += [] if stem == "__init__" else [stem]
+            if parts and all(x.isidentifier() for x in parts):
+                return ".".join(parts), suffix, tag
+        return None
+
+
+def _imports(report, tree, roots, objs, model, path_of, sym_ids, resolver, version, arch, counted):
+    """The import check of check_entries(python=version): report["python"], problems and notes of kind "python" and
+    the stats modules, python_skipped, find_queries and find_ms.  counted: the resolver's (uploaded, downloaded)
+    bytes already in the report's stats."""
+    finder = _Finder(tree, version, arch)
+    problems, notes = report["problems"], report["notes"]
+    seen = {(p["object"], p["kind"], p["detail"]) for p in problems + notes}
+
+    def problem(obj, detail, weak=False):
+        if (obj, "python", detail) not in seen:
+            seen.add((obj, "python", detail))
+            (notes if weak else problems).append({"object": obj, "kind": "python", "detail": detail})
+
+    def what(spec):
+        if spec is None:
+            return "no module"
+        return spec[0] if spec[0] is not None else "the namespace package " + ":".join(spec[1])
+
+    path_by_id = {sid[0]: posixpath.normpath(path_of[k]) for k, sid in sym_ids.items()}
+    modules, queries, qmeta, flat, scopes, skipped = {}, [], [], [], {}, 0
+    for root_path, key in roots:
+        p = posixpath.normpath(root_path)
+        if not any(p.startswith(e + "/") for e in finder.entries):
+            continue
+        got = finder.name(p)
+        rec = {"module": None, "class": "library", "export": None, "defined_by": None, "status": None}
+        modules[p] = rec
+        if got is None:
+            continue
+        module, suffix, tag = got
+        spec = finder.find(module)
+        rec["module"] = module
+        if tag is not None:
+            rec["class"] = "other python"
+            if spec is None:
+                problem(p, "%s: built only for %s; Python %s finds no module %s" % (module, tag, version, module))
+            else:
+                problem(p, "%s: built for %s, which Python %s does not load; it imports %s"
+                        % (module, tag, version, what(spec)), True)
+            continue
+        if spec is None or spec[0] is None or tree.lookup(spec[0]) != key:
+            rec["class"] = "shadowed"
+            problem(p, "%s: never loaded: Python %s imports %s" % (module, version, what(spec)), True)
+            continue
+        rec["class"], rec["export"] = "module", export_name(module).decode("ascii")
+        loaded, resolutions, _ = model.closure(root_path, key)
+        if any(r[3] == "missing" for r in resolutions) or any(objs[k].status != N.ELF_OK for _, k in loaded) or \
+                sym_ids[key][1] != N.SYM_OK:
+            rec["status"] = "not checked"
+            skipped += 1
+            continue
+        ids = tuple(sym_ids[k][0] for _, k in loaded)  # provided libraries are not read: they define no PyInit_*
+        if ids not in scopes:
+            scopes[ids] = len(flat)
+            flat += ids
+        queries.append((scopes[ids], len(ids), export_name(module)))
+        qmeta.append((p, suffix))
+    ms0 = resolver.stats().get("find_ms", 0.0)
+    for (p, suffix), (obj, _, _, _, _) in zip(qmeta, resolver.find(queries, flat)):
+        rec = modules[p]
+        if obj is not None:
+            rec["status"], rec["defined_by"] = "ok", path_by_id[obj]
+        elif suffix == ".so":  # a bare .so without the export: a library that happens to be importable by name
+            rec.update({"module": None, "class": "library", "export": None})
+        else:
+            rec["status"] = "not exported"
+            problem(p, '%s not exported: the import fails with "dynamic module does not define module export function"'
+                    % rec["export"])
+    st = report["stats"]
+    st["bytes_up"] += resolver.uploaded - counted[0]
+    st["bytes_down"] += resolver.downloaded - counted[1]
+    st.update({"modules": sum(1 for r in modules.values() if r["class"] == "module"), "python_skipped": skipped,
+               "find_queries": len(queries), "find_ms": resolver.stats().get("find_ms", 0.0) - ms0})
+    report["python"] = {"version": version, "path": finder.path, "modules": dict(sorted(modules.items()))}
+
+
 def check_zip(zip_path, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVIDED, max_versions=None,
               ld_library_path=LAMBDA_LD_LIBRARY_PATH, ctx=None, batch_bytes=BATCH_BYTES, *, symbols=False,
-              interpreter=(), runtime_libs=()):
+              interpreter=(), runtime_libs=(), python=None):
     """Check that the shared objects of `zip_path`, unpacked at `mount`, will load on Lambda (see the module docstring
     for the search it restates).  Returns a plain dict:
 
@@ -835,20 +1075,31 @@ def check_zip(zip_path, mount="/var/task", arch="x86_64", provided=DEFAULT_PROVI
     refs and resolve kernels, CUDA events; also split as symbols_index_ms, symbols_refs_ms, symbols_resolve_ms),
     references, lookups and symbols_skipped (roots with a missing need or an unloadable object, not checked).
 
+    python="3.N" (3.8 .. 3.14) also checks that the extension modules will import on that Python (DESIGN.md section
+    9.11): CPython's finder restated on LAMBDA_PYTHON_PATH's entries under `mount`, with the target's suffixes
+    (.cpython-3N-<arch triplet>.so, .abi3.so, .so, then .py, .pyc), and each module's PyInit_<name> looked up in its
+    load scope as dlsym looks it up.  The report gains python {version, path (the sys.path modelled), modules {mounted
+    path of every *.so under a path entry: module (dotted name), class ("module", "shadowed", "other python",
+    "library"), export, defined_by, status ("ok", "not exported", "not checked"; modules only)}}, problems of kind
+    "python" (a build only for another Python whose name the finder does not find; a module without its PyInit_*),
+    notes of kind "python" (a shadowed file; a build for another Python beside one that loads) and stats modules,
+    python_skipped (modules with a missing need or an unloadable object, not looked up), find_queries and find_ms.
+
     Members are inflated by the GPU zip reader and parsed on the GPU (lb2_elf_deps) where they lie; only the records
     and their strings come back.  There is no CPU path: without a GPU this raises."""
     from .tarball import _default_context
     own = False
     if ctx is None:
         ctx, own = _default_context()
+    python_version(python)
     try:
         with Z.GpuUnzipDecoder(ctx) as dec, GpuElfParser(ctx) as parser:
-            if not symbols:
+            if not symbols and not python:
                 return check_with(zip_path, dec, parser, mount, arch, provided, max_versions, ld_library_path, batch_bytes)
             with GpuSymbolResolver(ctx) as resolver:
                 return check_with(zip_path, dec, parser, mount, arch, provided, max_versions, ld_library_path,
-                                  batch_bytes, symbols=True, interpreter=interpreter, runtime_libs=runtime_libs,
-                                  resolver=resolver)
+                                  batch_bytes, symbols=symbols, interpreter=interpreter, runtime_libs=runtime_libs,
+                                  resolver=resolver, python=python)
     finally:
         if own:
             ctx.close()
@@ -865,6 +1116,9 @@ def summary(report):
     if "symbols" in report:
         lines.append("symbols: %d references, %d lookups, %d root(s) not checked"
                      % (st["references"], st["lookups"], st["symbols_skipped"]))
+    if "python" in report:
+        lines.append("python %s: %d extension modules, %d not checked, %d PyInit lookups"
+                     % (report["python"]["version"], st["modules"], st["python_skipped"], st["find_queries"]))
     for p in report["problems"]:
         lines.append("problem: %s: %s: %s" % (p["object"], p["kind"], p["detail"]))
     for p in report["notes"]:
@@ -893,17 +1147,21 @@ def add_check_arguments(ap):
                     help="with --symbols: an ELF file heading the global scope, such as the python executable (repeatable)")
     ap.add_argument("--runtime-lib", action="append", default=[], metavar="DIR",
                     help="with --symbols: a directory holding the runtime's provided libraries (repeatable)")
-    return ("mount", "arch", "provided", "max_version", "ld_library_path", "symbols", "interpreter", "runtime_lib")
+    ap.add_argument("--python", metavar="3.N", help="also check that the extension modules import on this Python "
+                                                    "(%s .. %s)" % (PYTHON_VERSIONS[0], PYTHON_VERSIONS[-1]))
+    return ("mount", "arch", "provided", "max_version", "ld_library_path", "symbols", "interpreter", "runtime_lib",
+            "python")
 
 
 def check_kwargs(args):
     """check_zip's keyword arguments from the options add_check_arguments defined; ValueError for a --max-version
-    that is not PREFIX_VERSION"""
+    that is not PREFIX_VERSION or a --python that is not one of PYTHON_VERSIONS"""
     return dict(mount=args.mount, arch=args.arch,
                 provided=DEFAULT_PROVIDED if args.provided is None else frozenset(args.provided),
                 max_versions=dict(_ceiling(t) for t in args.max_version), ld_library_path=args.ld_library_path,
                 **({"symbols": True, "interpreter": args.interpreter, "runtime_libs": args.runtime_lib}
-                   if args.symbols else {}))
+                   if args.symbols else {}),
+                **({"python": python_version(args.python)} if args.python is not None else {}))
 
 
 def main(argv=None, check=check_zip):

@@ -358,8 +358,8 @@ def _check_engines(check, parser, resolver):
     if check is None:
         return None
     check = D.check_options(check)
-    if parser is None or (check.get("symbols") and resolver is None):
-        raise ValueError("check needs a parser, and a resolver with symbols=True")
+    if parser is None or ((check.get("symbols") or check.get("python")) and resolver is None):
+        raise ValueError("check needs a parser, and a resolver with symbols=True or python")
     return check
 
 
@@ -429,7 +429,7 @@ def zip_tarballs(srcs, dst, prefix="", ctx=None, compresslevel=None, fallback_ho
     index, inflate, strip and deflate (the engines' stats) and kernel_ms, their kernel times summed.
 
     check (a dict of check_zip's keyword arguments: mount, arch, provided, max_versions, ld_library_path, symbols,
-    interpreter, runtime_libs) checks the zip before it is written, on the stripped objects where they lie on the
+    interpreter, runtime_libs, python) checks the zip before it is written, on the stripped objects where they lie on the
     device (DESIGN.md section 9.10): stats["check"] is the report check_zip(dst, **check) would return, with stats
     roots_reused added, and a report with problems raises deps.CheckFailed (its report attached) before dst is
     created or replaced.  An unknown key or a refused value raises ValueError before any source is read.  There is
@@ -457,7 +457,8 @@ def _check_engine_set(ctx, check):
     """(GpuElfParser, GpuSymbolResolver) for check, each None where check does not need it"""
     with contextlib.ExitStack() as stack:
         parser = stack.enter_context(D.GpuElfParser(ctx)) if check is not None else None
-        resolver = stack.enter_context(D.GpuSymbolResolver(ctx)) if check is not None and check.get("symbols") else None
+        resolver = stack.enter_context(D.GpuSymbolResolver(ctx)) \
+            if check is not None and (check.get("symbols") or check.get("python")) else None
         yield parser, resolver
 
 
@@ -1095,8 +1096,8 @@ def main(argv=None):
     if not args.srcs and not args.wheel:
         ap.error("give at least one tarball or --wheel")
     if not args.check and any(getattr(args, k) != ap.get_default(k) for k in check_dests):
-        ap.error("--mount, --arch, --provided, --max-version, --ld-library-path, --symbols, --interpreter and "
-                 "--runtime-lib need --check")
+        ap.error("--mount, --arch, --provided, --max-version, --ld-library-path, --symbols, --interpreter, "
+                 "--runtime-lib and --python need --check")
     try:
         kw = {"check": D.check_kwargs(args)} if args.check else {}
         if args.wheel or args.clean:
